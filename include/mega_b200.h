@@ -1,4 +1,4 @@
-/* mega_b200.h -- C ABI of libmega_b200.so: hand-written sm_100a kernels for the MEGA
+/* mega_b200.h -- C ABI of libmega_b200.so: hand-written sm_90a (H100) kernels for the MEGA
  * (Scalsol/mega.pytorch) per-frame inference hot path.
  *
  * Conventions
@@ -26,14 +26,14 @@ extern "C" {
 /* ------------------------------------------------------------------ library */
 const char* mega_last_error(void);
 int mega_abi_version(void);
-/* 1 if the current CUDA device is sm_100 (B200), 0 otherwise, <0 on CUDA error. */
+/* 1 if the current CUDA device is sm_90 (H100), 0 otherwise, <0 on CUDA error. */
 int mega_device_ok(void);
 
-/* ------------------------------------------------- dense contractions (tcgen05)
- * Implicit-GEMM convolution / GEMM on the tensor cores, FP32 accumulation in TMEM. Operand arithmetic is selected
+/* ------------------------------------------------- dense contractions (wgmma)
+ * Implicit-GEMM convolution / GEMM on the tensor cores, FP32 accumulation in registers. Operand arithmetic is selected
  * by `precision`: 0 = fp32 tensors rounded to TF32 on load, 1 = fp32 tensors, 3xTF32 split (near-fp32), 2 = fp16
  * tensors (same 10-bit mantissa as TF32, half the bytes, twice the tensor-pipe rate), 3 = "3xFP16": operands in the
- * SPLIT-FP16 format (below; near-fp32 like 1, kind::f16 MMAs, no split work in the kernel); the output / residual are
+ * SPLIT-FP16 format (below; near-fp32 like 1, f16 MMAs, no split work in the kernel); the output / residual are
  * fp32, or fp16 when out_f16 != 0 (precision 2), or split-fp16 (precision 3: out_f16 != 0 for the output, res_split != 0
  * for the residual).
  * SPLIT-FP16 format: a tensor with the shape, strides and byte size of an fp32 tensor whose innermost dimension is a
@@ -152,13 +152,10 @@ int mega_conv_chain_launch2(const void* plan_device, int n_layers, int grid, voi
 int mega_conv_chain_set_trace(void* trace_dev, int cta);
 /* level 1: per-layer events only, so that a 100-layer chain fits the buffer (tools/trace_backbone.py) */
 int mega_conv_chain_set_trace2(void* trace_dev, int cta, int level);
-/* 3xTF32 (precision 1): the tensor core adds into its fp32 TMEM accumulator with truncation, a bias that grows with
+/* 3xTF32 (precision 1): the tensor core adds into its fp32 accumulator with truncation, a bias that grows with
  * the number of MMAs accumulated; the kernel restarts the accumulator every `k_blocks` k-blocks (12 MMAs each) and folds
  * the segments into a master accumulator with round-to-nearest adds. 1..64, default 2; returns the previous value. */
 int mega_set_split3_seg_len(int k_blocks);
-/* precision 3: 1 = the A operand goes through tensor memory (tcgen05.cp per staged tile, TS-form MMAs; same results), 0 = both
- * operands from shared memory. Returns the previous setting. */
-int mega_set_split16_a_tmem(int enable);
 /* TMA fp32->tf32 conversion on load (round-to-nearest) on/off; returns the previous value. */
 int mega_set_tf32_rounding(int enable);
 

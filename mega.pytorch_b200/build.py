@@ -1,4 +1,4 @@
-"""Builds lib/libmega_b200.so (the C-ABI CUDA library) with nvcc for sm_100a.
+"""Builds lib/libmega_b200.so (the C-ABI CUDA library) with nvcc for sm_90a (H100).
 
 Usage: python build.py [--force] [--verbose]
 The library has no torch / CUTLASS dependency; cudart is linked statically, so it loads on a
@@ -17,7 +17,7 @@ LIB = os.path.join(LIBDIR, "libmega_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
     "--threads", "8",

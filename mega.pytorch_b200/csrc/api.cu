@@ -13,11 +13,11 @@ void mega_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* mega_last_error(void) { return g_err; }
-extern "C" int mega_abi_version(void) { return 6; }
+extern "C" int mega_abi_version(void) { return 7; }
 extern "C" int mega_device_ok(void) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return -1;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return -1;
-  return (prop.major == 10 && prop.minor == 0) ? 1 : 0;
+  return (prop.major == 9 && prop.minor == 0) ? 1 : 0;
 }

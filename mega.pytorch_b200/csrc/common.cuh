@@ -1,5 +1,5 @@
-// Common device/host helpers for the sm_100a kernels of the MEGA hot path.
-// Everything here is inline PTX for Blackwell (tcgen05 / TMEM / TMA / mbarrier);
+// Common device/host helpers for the sm_90a kernels of the MEGA hot path.
+// Everything here is inline PTX for Hopper (wgmma / TMA / mbarrier);
 // there is no dependency on CUTLASS or torch.
 #pragma once
 #include <cuda.h>
@@ -90,7 +90,8 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// Bounded wait: a pipeline bug traps after ~2 s instead of hanging the GPU box.
+// Bounded wait: a pipeline bug traps after ~2 s instead of hanging the GPU. No report is printed: printf is a function
+// call, and a call anywhere in a kernel that issues wgmma makes ptxas serialise every one of its wgmma groups.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
 #ifndef MEGA_NO_WATCHDOG
@@ -99,11 +100,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 #endif
   while (!mbar_try_wait(bar, parity)) {
 #ifndef MEGA_NO_WATCHDOG
-    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > 2000000000ull) {
-      printf("mega: mbarrier wait timeout block(%d,%d,%d) thread %d parity %u\n", blockIdx.x,
-             blockIdx.y, blockIdx.z, threadIdx.x, parity);
-      __trap();
-    }
+    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > 2000000000ull) __trap();
 #endif
   }
 }
@@ -155,135 +152,31 @@ __device__ __forceinline__ void tma_store_wait() {
 // make generic-proxy smem writes visible to the async proxy (TMA store reads them)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ----------------------------------------------------------------- tcgen05 --
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ------------------------------------------------------------------- wgmma --
+// order register / shared-memory accesses of this warpgroup before the wgmma.mma_async that follow
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// at most N committed wgmma groups of this warpgroup still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T ; operands described by 64-bit smem descriptors.
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// TS form: the A operand (128 rows x 8 tf32 of K) is read from TENSOR MEMORY (lane = row, 8 consecutive 32-bit columns
-// from tmem_a), B from shared memory through its descriptor.
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// shared memory -> tensor memory: the 128-row x 256-bit matrix slice named by a shared-memory matrix descriptor (the one an
-// SS-form MMA would read its A operand through) into lanes 0..127 x 8 columns starting at taddr; asynchronous, ordered with
-// the tcgen05.mma / tcgen05.cp instructions the same thread issues before and after it
-__device__ __forceinline__ void tmem_cp_128x256b(uint32_t taddr, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-}
-// mbarrier arrive once every MMA issued so far by this thread has completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread t of the warp receives lane (base+t), columns c..c+31.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_wait_regs(float (&d)[N]) {
+  // the accumulators are read by ordinary instructions next: they must not be moved across the wait
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // K-major operand tile stored as rows of exactly 128 bytes with the 128B swizzle
 // (what TMA writes for a box whose inner extent is 128 B): 8-row groups are 1024 B apart.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
+// Advancing the start address by 32 B selects the next 32 bytes of K inside the swizzle row.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);  // start address, 16 B units
   d |= static_cast<uint64_t>(1) << 16;                  // leading byte offset (unused for SW128 K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;          // stride byte offset: 8 rows * 128 B
-  d |= static_cast<uint64_t>(1) << 46;                  // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                  // layout: SWIZZLE_128B
-  return d;
-}
-
-// instruction descriptor: fp32 accumulate, K-major A and B, M x N tile
-template <int kFormat /*0=f16 1=bf16 2=tf32*/>
-__device__ __forceinline__ uint32_t umma_idesc(int m, int n) {
-  uint32_t d = 0;
-  d |= 1u << 4;                          // D format = F32
-  d |= static_cast<uint32_t>(kFormat) << 7;   // A format
-  d |= static_cast<uint32_t>(kFormat) << 10;  // B format
-  d |= static_cast<uint32_t>(n >> 3) << 17;
-  d |= static_cast<uint32_t>(m >> 4) << 24;
+  d |= static_cast<uint64_t>(1) << 62;                  // layout: SWIZZLE_128B
   return d;
 }
 

@@ -3,39 +3,42 @@
 // The backbone of the MEGA hot path is a strictly sequential chain of ~100 small implicit GEMMs per frame pair
 // (ResNet-101 res2..res5, modeling/backbone/resnet.py:324-344; RPN head, rpn/rpn.py:99-106). Each of them is 2-10 us
 // of tensor-core work at M = 4788 output pixels, so one-kernel-per-layer execution is dominated by what surrounds
-// the math: launch, barrier/TMEM set-up, descriptor fetch, pipeline fill and drain (measured 17-30 us per layer,
-// profiles/r01_ncu_full_conv_gemm_f16_res4_raw.csv: tensor pipe active 4-10 % of the kernel's duration).
+// the math: launch, barrier set-up, descriptor fetch, pipeline fill and drain.
 //
-// Here the per-layer kernel body (TMA producer warp / tcgen05 MMA warp / 8 epilogue warps, double-buffered TMEM
-// accumulators, persistent stream-K work list -- see conv_gemm_kernel.cuh) is wrapped in a loop over a device-side
-// table of layers. One CTA per SM stays resident for the whole chain; mbarriers, the TMEM allocation and the smem
-// ring are set up once; layers are separated by a grid-wide barrier (one atomic counter, release/acquire) instead of
-// a kernel boundary. Tensor maps live in the layer table in global memory.
+// Here the per-layer kernel body (TMA producer warp / two wgmma warpgroups / 8 epilogue warps fed through the
+// accumulator ring, persistent stream-K work list -- see conv_gemm_kernel.cuh) is wrapped in a loop over a device-side
+// table of layers. One CTA per SM stays resident for the whole chain; mbarriers and the smem rings are set up once;
+// layers are separated by a grid-wide barrier (one atomic counter, release/acquire) instead of a kernel boundary.
+// Tensor maps live in the layer table in global memory.
 //
 // Barrier depth. With depth 1 layer l starts when every CTA has finished layer l-1: the tensor pipe idles through every
-// layer's tail (last epilogue ~2.2 us, store drain + gpu-scope release ~1 us, barrier ~0.8 us, first operand fetch
-// ~0.8 us: 5-6 us against 3-10 us of MMAs per ResNet-101 layer at two 600x1000 frames -- tools/trace_chain.py). With
-// depth 2 layer l only waits for layer l-2 (one arrival counter per layer parity), so a table that INTERLEAVES two
+// layer's tail (last epilogue, store drain + gpu-scope release, barrier, first operand fetch). With depth 2 layer l only waits for layer l-2 (one arrival counter per layer parity), so a table that INTERLEAVES two
 // independent chains A0 B0 A1 B1 ... (the per-frame branch of two halves of an image batch) keeps the TMA / MMA warps of
 // every CTA streaming chain B's layer while chain A's tail drains, and vice versa. Stream-K partial sums and tile
 // counters of odd layers live in the second half of the workspace (a CTA may already publish partials of layer l+1
 // while a slower CTA still reduces layer l).
 //
-// Restrictions of a chain: fp16 operands (kind::f16), block_n <= 128 (one 32 KB smem stage holds A 128 x 64 and B
+// Restrictions of a chain: fp16 operands, block_n <= 128 (one 32 KB smem stage holds A 128 x 64 and B
 // block_n x 64 halves), output fp16 or fp32 per layer.
 #include "conv_gemm_kernel.cuh"
 
 namespace mega {
 
-constexpr int kChainStages = 5;
+constexpr int kChainStages = 4;
 constexpr int kChainStageBytes = 32768;     // A tile 16 KB + B tile (<= 128 rows) 16 KB
 constexpr int kChainABytes = 16384;
+constexpr int kChainRingOffset = kChainStages * kChainStageBytes;
+constexpr int kChainEpiOffset = kChainRingOffset + kRingSlots * kRingSlotBytes;
 constexpr int kChainEpiBytes = 4 * 4 * 4096;
-constexpr int kChainBarOffset = kChainStages * kChainStageBytes + kChainEpiBytes;
+constexpr int kChainBarOffset = kChainEpiOffset + kChainEpiBytes;
 constexpr int kChainSbOffset = kChainBarOffset + 256;      // [scale | bias][128] floats of the tile being finished
 constexpr int kChainSmem = kChainSbOffset + 1024 + 1024;
-constexpr uint32_t kChainTmemCols = 256;    // two accumulators of up to 128 fp32 columns
-constexpr uint32_t kChainAccStride = 128;
+static_assert(kChainSmem <= 227 * 1024, "chain pipeline + staging exceed the 227 KB of a CTA");
+struct ChainSmemLayout {     // what mma_pass needs to know of a stage
+  static constexpr int kStageBytes = kChainStageBytes;
+  static constexpr int kABytes = kChainABytes;
+  static constexpr int kBBytes = kChainStageBytes - kChainABytes;
+};
 
 struct alignas(128) ChainLayer {
   CUtensorMap tmA, tmB, tmOut, tmRes;
@@ -66,11 +69,7 @@ __device__ __forceinline__ void grid_wait(const unsigned* ctr, unsigned target) 
   uint32_t spins = 0;
   while (ld_acquire_u32(ctr) < target) {
     __nanosleep(40);
-    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > 2000000000ull) {
-      printf("mega: chain grid barrier timeout block %d thread %d target %u have %u\n", blockIdx.x, threadIdx.x, target,
-             ld_acquire_u32(ctr));
-      __trap();
-    }
+    if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > 2000000000ull) __trap();   // (no printf: see mbar_wait)
   }
   fence_proxy_async_all();
 }
@@ -80,7 +79,7 @@ struct PipeState {
   uint32_t phase;
 };
 
-// optional in-kernel event trace of ONE CTA (diagnostics, tools/trace_chain.py): (tag, SM clock) pairs per role
+// optional in-kernel event trace of ONE CTA (diagnostics): (tag, SM clock) pairs per role
 struct ChainTrace {
   unsigned long long* buf;   // [3 roles][kTraceCap][2] or NULL
   int cta;
@@ -113,20 +112,18 @@ __device__ __forceinline__ TraceCursor trace_cursor(const ChainTrace& tr, int ro
 #define TR_TAG(layer, idx, code) ((static_cast<unsigned long long>(layer) << 32) | (static_cast<unsigned long long>(idx) << 8) | (code))
 
 // ------------------------------------------------------------------ epilogue of one layer (8 warps)
-// Eight epilogue warps: warp w reads TMEM lane quarter (w & 3) (the hardware restriction: a warp touches lanes
-// 32*(warp_id % 4) .. +31), and of the tile's 64-column (fp16 out) / 32-column (fp32 out) chunks it takes those with
-// chunk % 2 == (w - 2) / 4. Round 1 ran 4 warps over all chunks with ~300 executed instructions per 32 columns (generic
-// LD / ST to the staging buffers, per-element branches on the layer's flags, FMUL + FMNMX for every ReLU): 4.1 us per
-// 128 x 128 tile with a residual against 1.2 us of MMAs for K = 256 (tools/trace_backbone.py), which made every
-// 1x1-expand layer of the backbone epilogue-bound. Here the flags are template parameters of the inner loop, staging
-// goes through explicit ld/st.shared with precomputed swizzled offsets, and two warps share a lane quarter.
-// (Tried on top and reverted: walking the work list one tile ahead to prefetch the next tile's scale / bias into registers
-// and its residual chunk by TMA. The residual still arrived 0.5 us after the accumulator -- it queues behind the main
-// loop's operand loads in the SM's TMA FIFO -- and the second decode_tile per tile cost more than the barriers it saved:
-// backbone chain 1.61 -> 1.70 ms at 2 images, 3.75 -> 4.04 ms at 8.)
+// Eight epilogue warps: warp w finishes tile rows 32 (w & 3) .. +31, and of the tile's 64-column (fp16 out) / 32-column
+// (fp32 out) chunks it takes those with chunk % 2 == (w - 2) / 4, so every accumulator ring slot is read by the four warps
+// of one parity. The layer's flags are template parameters of the inner loop, staging goes through explicit ld/st.shared
+// with precomputed swizzled offsets, and two warps share a row quarter.
 constexpr int kEpiWarps = 8;
 constexpr int kEpiThreads = kEpiWarps * 32;
-constexpr int kChainThreads = 64 + kEpiThreads;
+// warps 0..7: the two MMA warpgroups; 8..15: epilogue; 16: TMA producer. 544 threads leave 120 registers per thread, which
+// the MMA warpgroups need to keep a 64 x 128 accumulator live across their asynchronous wgmma groups
+constexpr int kChainMmaWarp0 = 0;
+constexpr int kChainEpiWarp0 = 8;
+constexpr int kChainProducerWarp = 16;
+constexpr int kChainThreads = (kChainProducerWarp + 1) * 32;
 
 __device__ __forceinline__ void epi_bar_sync_all() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
@@ -215,18 +212,19 @@ __device__ __forceinline__ void epi_half_dispatch(const uint32_t (&raw)[32], uin
 }
 
 template <bool OUT16>
-__device__ __noinline__ void chain_epilogue_layer(const ChainLayer* L, const ConvGemmParams& p, const int BN, uint8_t* smem,
-                                                  uint64_t* tmem_full_bar, uint64_t* tmem_empty_bar, uint64_t* res_bar,
-                                                  int* epi_flag, uint32_t tmem_base, int warp, int lane, int cta,
-                                                  int grid, int& item, uint32_t& rphase, TraceCursor& tr, int layer) {
+__device__ __forceinline__ void chain_epilogue_layer(const ChainLayer* L, const ConvGemmParams& p, const int BN, uint8_t* smem,
+                                                  uint64_t* ring_full, uint64_t* ring_empty, uint64_t* res_bar,
+                                                  int* epi_flag, int warp, int lane, int cta,
+                                                  int grid, uint32_t& ruse, uint32_t& rphase, TraceCursor& tr, int layer) {
   constexpr int CW = OUT16 ? 64 : 32;          // columns per chunk (= one 128-byte staging row)
   constexpr int HPC = CW / 32;                 // 32-column halves per chunk
-  const int ew = warp - 2;                     // epilogue warp 0..7
-  const int q = warp & 3;                      // TMEM lane quarter
+  const int ew = warp - kChainEpiWarp0;        // epilogue warp 0..7
+  const int q = warp & 3;                      // 32-row quarter of the tile
   const int half = ew >> 2;                    // parity of the chunks this warp takes
   const int row = q * 32 + lane;
   const int epi_tid = ew * 32 + lane;
-  const uint32_t stage_base = smem_u32(smem + kChainStages * kChainStageBytes + ew * 8192);
+  const uint32_t stage_base = smem_u32(smem + kChainEpiOffset + ew * 8192);
+  const uint8_t* ring = smem + kChainRingOffset;
   const uint32_t out_row = stage_base + lane * 128;          // 4 KB store staging | 4 KB residual staging per warp
   const uint32_t res_row = out_row + 4096;
   uint64_t* rbar = res_bar + ew;
@@ -234,7 +232,6 @@ __device__ __noinline__ void chain_epilogue_layer(const ChainLayer* L, const Con
   float* sb_s = reinterpret_cast<float*>(smem + kChainSbOffset);
   const int U = static_cast<int>(p.total_units);
   const int KB = p.kb_per_tile;
-  const uint32_t lane_bits = static_cast<uint32_t>(q * 32) << 16;
   const CUtensorMap* tmOut = &L->tmOut;
   const CUtensorMap* tmRes = &L->tmRes;
   const bool has_res = p.has_residual != 0;
@@ -245,11 +242,9 @@ __device__ __noinline__ void chain_epilogue_layer(const ChainLayer* L, const Con
   WorkIter it(p, cta, grid);
   int t;
   int kb0, kb1;
+  // every 32-column accumulator chunk of this warp's epilogue chunks arrives in ring slot `half`; ruse counts them
   for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item) {
     const TileCoord tc = decode_tile(p, t, BN);
-    const int buf = item & 1;
-    const uint32_t use = static_cast<uint32_t>(item >> 1);
-    ++item;
     const bool complete = (kb0 == 0 && kb1 == KB);
     const int r0 = q * 32;
     const int bh0 = r0 / p.tile_w, bw0 = r0 - bh0 * p.tile_w;
@@ -267,14 +262,11 @@ __device__ __noinline__ void chain_epilogue_layer(const ChainLayer* L, const Con
     }
     if (complete && has_res && lane == 0 && half < nchunks) {
       mbar_arrive_expect_tx(rbar, 4096);
-      tma_load_4d(reinterpret_cast<void*>(smem + kChainStages * kChainStageBytes + ew * 8192 + 4096), tmRes, rbar,
+      tma_load_4d(reinterpret_cast<void*>(smem + kChainEpiOffset + ew * 8192 + 4096), tmRes, rbar,
                   tc.n0 + half * CW + tc.batch * p.res_c_off, st_w, st_h, res_n);
     }
     epi_bar_sync_all();
-    mbar_wait(&tmem_full_bar[buf], use & 1);
-    tc_fence_after();
     tr.put(TR_TAG(layer, tile_item, 4));
-    const uint32_t tmem_row = tmem_base + buf * kChainAccStride + lane_bits;
     bool finalize = complete;
     int c_first = cta, c_last = cta;
     if (!complete) {
@@ -285,9 +277,7 @@ __device__ __noinline__ void chain_epilogue_layer(const ChainLayer* L, const Con
         for (int h = 0; h < HPC; ++h) {
           const int g32 = c * HPC + h;
           uint32_t acc[32];
-          __syncwarp();
-          tmem_ld_32x32(tmem_row + g32 * 32, acc);
-          tmem_ld_wait();
+          ring_take(ring, ring_full, ring_empty, half, ruse++, row, acc);
 #pragma unroll
           for (int j = 0; j < 32; j += 4) {
             float4 v = make_float4(__uint_as_float(acc[j]), __uint_as_float(acc[j + 1]), __uint_as_float(acc[j + 2]),
@@ -319,7 +309,7 @@ __device__ __noinline__ void chain_epilogue_layer(const ChainLayer* L, const Con
         if (has_res) {
           if ((!complete || c != half) && lane == 0) {   // (whole tiles started their first load before the MMAs)
             mbar_arrive_expect_tx(rbar, 4096);
-            tma_load_4d(reinterpret_cast<void*>(smem + kChainStages * kChainStageBytes + ew * 8192 + 4096), tmRes, rbar,
+            tma_load_4d(reinterpret_cast<void*>(smem + kChainEpiOffset + ew * 8192 + 4096), tmRes, rbar,
                         nb + tc.batch * p.res_c_off, st_w, st_h, res_n);
           }
           mbar_wait(rbar, (rphase >> ew) & 1u);
@@ -333,26 +323,20 @@ __device__ __noinline__ void chain_epilogue_layer(const ChainLayer* L, const Con
         for (int h = 0; h < HPC; ++h) {
           const int col0 = c * CW + h * 32;     // first column of this half inside the tile
           uint32_t raw[32];
-          __syncwarp();
-          tmem_ld_32x32(tmem_row + col0, raw);
-          tmem_ld_wait();
-          if (!complete) {
-            // deterministic reduction: parts summed in CTA order, own part from TMEM
+          if (complete) {
+            ring_take(ring, ring_full, ring_empty, half, ruse++, row, raw);
+          } else {
+            // deterministic reduction: parts summed in CTA order (this CTA's own part as published above)
             float sum[32];
 #pragma unroll
             for (int j = 0; j < 32; ++j) sum[j] = 0.f;
             for (int oc = c_first; oc <= c_last; ++oc) {
-              if (oc == cta) {
+              const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
+              const float* ws = p.part_ws + ((static_cast<long long>(oc) * 2 + slot) * kBM + row) * BN + col0;
 #pragma unroll
-                for (int j = 0; j < 32; ++j) sum[j] += __uint_as_float(raw[j]);
-              } else {
-                const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
-                const float* ws = p.part_ws + ((static_cast<long long>(oc) * 2 + slot) * kBM + row) * BN + col0;
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                  const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + j));
-                  sum[j] += v.x; sum[j + 1] += v.y; sum[j + 2] += v.z; sum[j + 3] += v.w;
-                }
+              for (int j = 0; j < 32; j += 4) {
+                const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + j));
+                sum[j] += v.x; sum[j + 1] += v.y; sum[j + 2] += v.z; sum[j + 3] += v.w;
               }
             }
 #pragma unroll
@@ -363,15 +347,19 @@ __device__ __noinline__ void chain_epilogue_layer(const ChainLayer* L, const Con
         fence_async_smem();
         __syncwarp();
         if (lane == 0) {
-          tma_store_4d(tmOut, smem + kChainStages * kChainStageBytes + ew * 8192, nb + tc.batch * p.out_c_off, st_w, st_h,
+          tma_store_4d(tmOut, smem + kChainEpiOffset + ew * 8192, nb + tc.batch * p.out_c_off, st_w, st_h,
                        out_n);
           tma_store_commit();
         }
       }
     }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&tmem_empty_bar[buf]);
+    if (complete) {
+      // chunks of this warp's parity past cout: hand their ring slots back unread
+      const int c0 = nchunks + ((nchunks & 1) != half ? 1 : 0);
+      for (int c = c0; c < BN / CW; c += 2)
+#pragma unroll
+        for (int h = 0; h < HPC; ++h) ring_skip(ring, ring_full, ring_empty, half, ruse++, row);
+    }
     tr.put(TR_TAG(layer, tile_item, 6));
   }
 }
@@ -385,42 +373,36 @@ conv_chain_kernel(const ChainLayer* __restrict__ layers, const int n_layers, uns
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kChainBarOffset);
   uint64_t* empty_bar = full_bar + kChainStages;
-  uint64_t* tmem_full_bar = empty_bar + kChainStages;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;         // [2]
-  uint64_t* res_bar = tmem_empty_bar + 2;               // [8 epilogue warps]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bar + 8);
-  int* epi_flag = reinterpret_cast<int*>(tmem_slot + 1);
+  uint64_t* ring_full = empty_bar + kChainStages;       // [kRingSlots]
+  uint64_t* ring_empty = ring_full + kRingSlots;         // [kRingSlots]
+  uint64_t* res_bar = ring_empty + kRingSlots;           // [8 epilogue warps]
+  int* epi_flag = reinterpret_cast<int*>(res_bar + 8);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int grid = gridDim.x;
   const int cta = blockIdx.x;
 
-  if (warp == 1 && lane == 0) {
+  if (warp == kChainProducerWarp && lane == 31) {
     for (int s = 0; s < kChainStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);      // one arrival per MMA warp
     }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full_bar[b], 1);
-      mbar_init(&tmem_empty_bar[b], kEpiWarps);
+    for (int b = 0; b < kRingSlots; ++b) {
+      mbar_init(&ring_full[b], 256);    // every MMA thread
+      mbar_init(&ring_empty[b], 4);     // the four epilogue warps of one chunk parity
     }
     for (int b = 0; b < kEpiWarps; ++b) mbar_init(&res_bar[b], 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, kChainTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_wait();
   griddep_launch_dependents();
 
-  if (warp == 0) {
+  if (warp == kChainProducerWarp) {
     // ===================== TMA producer =====================
     // lane 0 loads the A (activation) tile and posts the expected byte count, lane 1 loads the B (weight) tile: the two
-    // descriptor-based copies of a k-block are issued in parallel (a single thread needs ~650 cycles per k-block for
-    // wait + expect + 2 TMA issues, measured with tools/trace_chain.py; the MMAs of a k-block take ~260)
+    // descriptor-based copies of a k-block are issued in parallel
     if (lane < 2) {
       PipeState ps = {0, 0};
       TraceCursor tr = trace_cursor(trace, 0, cta);
@@ -483,54 +465,44 @@ conv_chain_kernel(const ChainLayer* __restrict__ layers, const int n_layers, uns
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      PipeState ps = {0, 0};
-      int item = 0;
-      TraceCursor tr = trace_cursor(trace, 1, cta);
-      for (int l = 0; l < n_layers; ++l) {
-        const ChainLayer* L = layers + l;
-        const ConvGemmParams p = L->p;
-        const int BN = L->block_n;
-        const int act = L->active_ctas;
-        int lc = cta - L->cta_rot;
-        if (lc < 0) lc += grid;
-        if (lc >= act) continue;
-        const uint32_t idesc = umma_idesc<0>(kBM, BN);
-        WorkIter it(p, lc, act);
-        int t;
-        int kb0, kb1;
-        while (it.next(t, kb0, kb1)) {
-          const int buf = item & 1;
-          const uint32_t use = static_cast<uint32_t>(item >> 1);
-          ++item;
-          mbar_wait(&tmem_empty_bar[buf], (use & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + buf * kChainAccStride;
-          for (int kb = kb0; kb < kb1; ++kb) {
-            mbar_wait(&full_bar[ps.stage], ps.phase);
-            tc_fence_after();
-            tr.put(TR_TAG(l, kb, 7));
-            const uint32_t a_addr = smem_u32(smem + ps.stage * kChainStageBytes);
-            const uint64_t adesc = umma_desc_sw128(a_addr);
-            const uint64_t bdesc = umma_desc_sw128(a_addr + kChainABytes);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_f16(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            umma_commit(&empty_bar[ps.stage]);
-            if (++ps.stage == kChainStages) {
-              ps.stage = 0;
-              ps.phase ^= 1;
-            }
-          }
-          umma_commit(&tmem_full_bar[buf]);
+  } else if (warp >= kChainMmaWarp0 && warp < kChainMmaWarp0 + 8) {
+    // ===================== MMA warpgroups =====================
+    const int wg = (warp - kChainMmaWarp0) >> 2;     // tile rows [64 wg, 64 wg + 64)
+    const int wtid = threadIdx.x - (kChainMmaWarp0 + 4 * wg) * 32;
+    MmaState ms = {0, 0, {0, 0}};
+    TraceCursor tr = trace_cursor(trace, 1, cta);
+    if (wtid != 0 || wg != 0) tr.p = nullptr;
+    uint8_t* ring = smem + kChainRingOffset;
+    for (int l = 0; l < n_layers; ++l) {
+      const ChainLayer* L = layers + l;
+      const ConvGemmParams p = L->p;
+      const int BN = L->block_n;
+      const int act = L->active_ctas;
+      int lc = cta - L->cta_rot;
+      if (lc < 0) lc += grid;
+      if (lc >= act) continue;
+      WorkIter it(p, lc, act);
+      int t;
+      int kb0, kb1;
+      const int hpc = L->out16 ? 2 : 1;       // 32-column chunks per epilogue chunk of this layer
+      while (it.next(t, kb0, kb1)) {
+        tr.put(TR_TAG(l, kb0, 7));
+        switch (BN) {
+          case 32: mma_pass<32, kChainStages, kModeF16, ChainSmemLayout>(smem, full_bar, empty_bar, empty_bar, ring, ring_full,
+                                                                          ring_empty, ms, kb0, kb1, 0x7fffffff, wg, wtid, hpc); break;
+          case 64: mma_pass<64, kChainStages, kModeF16, ChainSmemLayout>(smem, full_bar, empty_bar, empty_bar, ring, ring_full,
+                                                                          ring_empty, ms, kb0, kb1, 0x7fffffff, wg, wtid, hpc); break;
+          case 96: mma_pass<96, kChainStages, kModeF16, ChainSmemLayout>(smem, full_bar, empty_bar, empty_bar, ring, ring_full,
+                                                                          ring_empty, ms, kb0, kb1, 0x7fffffff, wg, wtid, hpc); break;
+          default: mma_pass<128, kChainStages, kModeF16, ChainSmemLayout>(smem, full_bar, empty_bar, empty_bar, ring, ring_full,
+                                                                           ring_empty, ms, kb0, kb1, 0x7fffffff, wg, wtid, hpc); break;
         }
       }
     }
-  } else {
-    // ===================== epilogue (warps 2..9) =====================
-    const int epi_tid = (warp - 2) * 32 + lane;
-    int item = 0;
+  } else if (warp >= kChainEpiWarp0 && warp < kChainEpiWarp0 + kEpiWarps) {
+    // ===================== epilogue (warps 8..15) =====================
+    const int epi_tid = (warp - kChainEpiWarp0) * 32 + lane;
+    uint32_t ruse = 0;    // chunks this warp took from its ring slot
     uint32_t rphase = 0;
     TraceCursor tr = trace_cursor(trace, 2, cta);
     if (epi_tid != 0) tr.p = nullptr;
@@ -553,11 +525,11 @@ conv_chain_kernel(const ChainLayer* __restrict__ layers, const int n_layers, uns
       if (lc < 0) lc += grid;
       if (lc < act) {
         if (L->out16) {
-          chain_epilogue_layer<true>(L, p, L->block_n, smem, tmem_full_bar, tmem_empty_bar, res_bar, epi_flag, tmem_base,
-                                     warp, lane, lc, act, item, rphase, tr, l);
+          chain_epilogue_layer<true>(L, p, L->block_n, smem, ring_full, ring_empty, res_bar, epi_flag,
+                                     warp, lane, lc, act, ruse, rphase, tr, l);
         } else {
-          chain_epilogue_layer<false>(L, p, L->block_n, smem, tmem_full_bar, tmem_empty_bar, res_bar, epi_flag, tmem_base,
-                                      warp, lane, lc, act, item, rphase, tr, l);
+          chain_epilogue_layer<false>(L, p, L->block_n, smem, ring_full, ring_empty, res_bar, epi_flag,
+                                      warp, lane, lc, act, ruse, rphase, tr, l);
         }
       }
       tr.put(TR_TAG(l, 0, 8));
@@ -582,13 +554,6 @@ conv_chain_kernel(const ChainLayer* __restrict__ layers, const int n_layers, uns
         __threadfence();
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kChainTmemCols);
   }
 }
 

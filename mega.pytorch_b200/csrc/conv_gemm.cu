@@ -1,5 +1,5 @@
-// Implicit-GEMM convolution / GEMM on the 5th-gen tensor cores (tcgen05, TF32 operands,
-// FP32 accumulate in TMEM), fed by TMA with the 128-byte shared-memory swizzle.
+// Implicit-GEMM convolution / GEMM on the Hopper tensor cores (wgmma, TF32 operands,
+// FP32 accumulate in registers), fed by TMA with the 128-byte shared-memory swizzle.
 //
 // One kernel serves every dense contraction of the MEGA hot path:
 //   * backbone / res5 / RPN-head convolutions (1x1, 3x3, 3x3 dilated) over NHWC maps
@@ -13,9 +13,9 @@
 // Tiling: the M tile is a th x tw rectangle of 128 output pixels, so the A operand of filter
 // tap (r,s) is the same rectangle shifted by (r,s)*dilation - pad: a plain 4-D tiled TMA load
 // with out-of-bounds zero fill supplies the padding. K is consumed in slabs of 32 floats
-// (= one 128 B swizzle row) per tap. Warp roles: warp 0 TMA producer, warp 1 MMA issuer,
-// warps 2-5 epilogue (TMEM -> registers -> global); the strict modes add warps 6-9: operand splitters (3xTF32) or a second
-// set of epilogue warps (3xFP16 on split-fp16 tensors, the mode the strict engine runs; see kModeF16x3 below).
+// (= one 128 B swizzle row) per tap. Warp roles: warp 0 TMA producer, two MMA warpgroups,
+// warps 2-5 epilogue (accumulator ring -> registers -> global); the strict modes add warps 6-9: operand splitters (3xTF32)
+// or a second set of epilogue warps (3xFP16 on split-fp16 tensors, the mode the strict engine runs; see conv_gemm_kernel.cuh).
 #include "conv_gemm_kernel.cuh"
 
 namespace mega {
@@ -42,7 +42,6 @@ static EncodeTiledFn get_encode_fn() {
 static int g_tf32_round = 1;  // TMA converts fp32 -> tf32 (round to nearest) while loading
 
 static int g_num_sms = 0;
-static int g_pk_a_tmem = 0;    // 3xFP16: A operand through tensor memory (tcgen05.cp + TS-form MMAs); mega_set_split16_a_tmem
 static int g_seg_len = 4;      // 3xTF32 / 3xFP16: k-blocks per accumulator segment (tools/strict_probe.py: 2 / 4 / 8 -> logits p99 1.8e-4 / 2.3e-4 / 5.3e-4)
 constexpr int kCounterSlots = 65536;   // ints at the head of the workspace
 constexpr int kMinUnits = 4;
@@ -59,12 +58,6 @@ extern "C" long long mega_conv_gemm_workspace_bytes(void) {
 extern "C" int mega_set_split3_seg_len(int k_blocks) {
   int old = g_seg_len;
   if (k_blocks >= 1 && k_blocks <= 64) g_seg_len = k_blocks;
-  return old;
-}
-
-extern "C" int mega_set_split16_a_tmem(int enable) {
-  int old = g_pk_a_tmem;
-  g_pk_a_tmem = enable ? 1 : 0;
   return old;
 }
 
@@ -186,7 +179,7 @@ int encode_conv_gemm_problem(const mega_conv_gemm_desc* d, CUtensorMap* tmA_p, C
     cuuint64_t gstr[2] = {static_cast<cuuint64_t>(d->b_stride_n) * esz,
                           static_cast<cuuint64_t>((taps > 1 || d->b_lo_tap_off) && d->b_stride_tap > 0
                                                       ? d->b_stride_tap : d->b_stride_n * d->b_n) * esz};
-    cuuint32_t box[3] = {static_cast<cuuint32_t>(bk), static_cast<cuuint32_t>(d->block_n), 1};
+    cuuint32_t box[3] = {static_cast<cuuint32_t>(bk), static_cast<cuuint32_t>(pass_n(d->block_n)), 1};   // one pass
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(&tmB, dt, 3, const_cast<void*>(d->b), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -283,7 +276,6 @@ int encode_conv_gemm_problem(const mega_conv_gemm_desc* d, CUtensorMap* tmA_p, C
   p.stream_k = d->stream_k ? 1 : 0;
   p.seg_len = g_seg_len;
   p.b_lo_tap_off = d->b_lo_tap_off;
-  p.a_tmem = (pk && g_pk_a_tmem) ? 1 : 0;
   p.res_split = d->res_split ? 1 : 0;
   p.acc_scale = (pk && d->acc_scale != 0.f) ? d->acc_scale : 1.f;
   MEGA_ARG_CHECK(tiles <= kCounterSlots, "conv_gemm: %lld output tiles exceed the %d counter slots", tiles, kCounterSlots);
@@ -334,16 +326,16 @@ extern "C" int mega_conv_gemm(const mega_conv_gemm_desc* d, void* stream_v) {
   if (f16) return launch_conv_gemm_f16(d->block_n, out16 ? 1 : 0, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
   if (strict) {
     return d->block_n == 64 ? launch_cfg<64, 4, kModeSplit3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
-                            : launch_cfg<128, 3, kModeSplit3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+                            : launch_cfg<128, 2, kModeSplit3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
   }
   switch (d->block_n) {
     case 32: return launch_cfg<32, 6, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    case 64: return launch_cfg<64, 6, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    case 96: return launch_cfg<96, 5, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    case 64: return launch_cfg<64, 5, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    case 96: return launch_cfg<96, 4, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
     case 128: return launch_cfg<128, 4, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    case 160: return launch_cfg<160, 4, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    case 160: return launch_cfg<160, 3, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
     case 192: return launch_cfg<192, 3, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    default: return launch_cfg<256, 3, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    default: return launch_cfg<256, 2, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
   }
 }
 

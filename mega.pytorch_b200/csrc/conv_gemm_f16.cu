@@ -1,5 +1,5 @@
-// fp16-operand instantiations of the tcgen05 implicit-GEMM kernel (conv_gemm_kernel.cuh): kind::f16 MMAs,
-// fp32 accumulation in TMEM, fp32 or fp16 output. Separate translation unit so nvcc builds it in parallel with
+// fp16-operand instantiations of the wgmma implicit-GEMM kernel (conv_gemm_kernel.cuh): f16 MMAs,
+// fp32 accumulation in registers, fp32 or fp16 output. Separate translation unit so nvcc builds it in parallel with
 // the TF32 variants.
 #include "conv_gemm_kernel.cuh"
 
@@ -18,12 +18,12 @@ int launch_conv_gemm_f16(int block_n, int out_f16, const CUtensorMap& tmA, const
                    : launch_cfg<BN, ST, kModeF16, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
   switch (block_n) {
     MEGA_F16_CASE(32, 6)
-    MEGA_F16_CASE(64, 6)
-    MEGA_F16_CASE(96, 5)
-    MEGA_F16_CASE(128, 5)
-    MEGA_F16_CASE(160, 4)
+    MEGA_F16_CASE(64, 5)
+    MEGA_F16_CASE(96, 4)
+    MEGA_F16_CASE(128, 4)
+    MEGA_F16_CASE(160, 3)
     MEGA_F16_CASE(192, 3)
-    MEGA_F16_CASE(256, 3)
+    MEGA_F16_CASE(256, 2)
   }
 #undef MEGA_F16_CASE
   mega_set_error("conv_gemm: unsupported block_n %d", block_n);

@@ -1,6 +1,6 @@
-// "3xFP16" instantiations of the tcgen05 implicit-GEMM kernel (conv_gemm_kernel.cuh, kModeF16x3): operands in the
-// split-fp16 format (include/mega_b200.h), three kind::f16 MMAs per k-step (hi.hi + hi.lo + lo.hi), fp32 accumulation in
-// TMEM in segments folded round-to-nearest, output fp32 or split-fp16. Own translation unit: built in parallel.
+// "3xFP16" instantiations of the wgmma implicit-GEMM kernel (conv_gemm_kernel.cuh, kModeF16x3): operands in the
+// split-fp16 format (include/mega_b200.h), three f16 MMAs per k-step (hi.hi + hi.lo + lo.hi), fp32 accumulation in
+// registers in segments folded round-to-nearest, output fp32 or split-fp16. Own translation unit: built in parallel.
 #include "conv_gemm_kernel.cuh"
 
 namespace mega {
@@ -9,12 +9,12 @@ int launch_conv_gemm_f16x3(int block_n, int out_split, const CUtensorMap& tmA, c
                            const CUtensorMap& tmOut, const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid,
                            cudaStream_t stream, int pdl) {
   if (block_n == 64) {
-    return out_split ? launch_cfg<64, 6, kModeF16x3, true>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
-                     : launch_cfg<64, 6, kModeF16x3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    return out_split ? launch_cfg<64, 5, kModeF16x3, true>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
+                     : launch_cfg<64, 5, kModeF16x3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
   }
   if (block_n == 128) {
-    return out_split ? launch_cfg<128, 5, kModeF16x3, true>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
-                     : launch_cfg<128, 5, kModeF16x3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    return out_split ? launch_cfg<128, 4, kModeF16x3, true>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
+                     : launch_cfg<128, 4, kModeF16x3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
   }
   mega_set_error("conv_gemm: 3xfp16 supports block_n 64 / 128 (got %d)", block_n);
   return MEGA_ERR_ARG;

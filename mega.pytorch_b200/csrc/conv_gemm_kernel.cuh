@@ -1,5 +1,5 @@
-// Implicit-GEMM convolution / GEMM on the 5th-gen tensor cores (tcgen05, TF32 operands,
-// FP32 accumulate in TMEM), fed by TMA with the 128-byte shared-memory swizzle.
+// Implicit-GEMM convolution / GEMM on the Hopper tensor cores (wgmma, TF32 / FP16 operands,
+// FP32 accumulate in registers), fed by TMA with the 128-byte shared-memory swizzle.
 //
 // One kernel serves every dense contraction of the MEGA hot path:
 //   * backbone / res5 / RPN-head convolutions (1x1, 3x3, 3x3 dilated) over NHWC maps
@@ -13,16 +13,18 @@
 // Tiling: the M tile is a th x tw rectangle of 128 output pixels, so the A operand of filter
 // tap (r,s) is the same rectangle shifted by (r,s)*dilation - pad: a plain 4-D tiled TMA load
 // with out-of-bounds zero fill supplies the padding. K is consumed in slabs of 32 floats
-// (= one 128 B swizzle row) per tap. Warp roles: warp 0 TMA producer, warp 1 MMA issuer,
-// warps 2-5 epilogue (TMEM -> registers -> global); the strict modes add warps 6-9: operand splitters (3xTF32) or a second
-// set of epilogue warps (3xFP16 on split-fp16 tensors, the mode the strict engine runs; see kModeF16x3 below).
+// (= one 128 B swizzle row) per tap. Warp roles: warp 0 TMA producer, warps 2-5 epilogue (accumulator ring -> registers
+// -> global); the strict modes add warps 6-9: operand splitters (3xTF32) or a second set of epilogue warps (3xFP16 on
+// split-fp16 tensors, the mode the strict engine runs; see kModeF16x3 below). Two MMA warpgroups follow the last of these
+// warps (kMmaWarp0): warpgroup g issues the wgmma of tile rows [64 g, 64 g + 64) and keeps that accumulator in registers.
 #include "common.cuh"
 #pragma once
 #include "mega_b200.h"
+#include "wgmma.cuh"
 
 namespace mega {
 
-constexpr int kBM = 128;        // UMMA M (one CTA)
+constexpr int kBM = 128;        // M tile of one CTA (two m64 warpgroups)
 // operand arithmetic of a launch
 constexpr int kModeTf32 = 0;    // fp32 operands in HBM, rounded to TF32 by the TMA load; K slab = 32 floats
 constexpr int kModeSplit3 = 1;  // "3xTF32": fp32 operands split hi/lo in shared memory
@@ -33,10 +35,22 @@ constexpr int kModeF16x3 = 3;   // "3xFP16": operands stored SPLIT in HBM -- eve
                                 // value as fp32 and 22 mantissa bits like 3xTF32, but NO split work in the kernel (the
                                 // producing epilogue / the weight packer did it) and kind::f16 MMAs; K slab = 32 values
 // every mode stages K slabs of 128 bytes per row (one swizzle row) and issues 4 MMAs of 32 bytes of K each
-// (3xFP16: 2 k-steps x 3 products over the hi / lo halves of the row)
+// (3xFP16: 2 k-steps x 3 products over the hi / lo halves of the row; 3xTF32: 4 k-steps x 3 products)
 __host__ __device__ constexpr int mode_bk(int mode) { return mode == kModeF16 ? 64 : 32; }
-constexpr int kThreads = 192;   // 6 warps
-constexpr int kMaxCtas = 148;   // persistent grid: one CTA per SM
+constexpr int kThreads = 192;   // 6 warps before the MMA warpgroups (10 in the strict modes)
+constexpr int kMaxCtas = 132;   // persistent grid: one CTA per SM of an H100 SXM
+// The MMA warpgroups hand finished accumulators to the epilogue warps through a ring of shared-memory slots of 32 columns
+// x 128 rows fp32 (row r = 128 bytes, 16-byte groups swizzled by r & 7: conflict-free for both sides). Every slot is read by
+// four epilogue warps (one per 32-row quarter) and produced in column order, tile after tile.
+constexpr int kRingSlots = 2;
+constexpr int kRingSlotBytes = kBM * 128;
+__host__ __device__ constexpr int mma_warp0(int mode) {
+  return (mode == kModeSplit3 || mode == kModeF16x3) ? 12 : 8;
+}
+__host__ __device__ constexpr int conv_gemm_threads(int mode) { return (mma_warp0(mode) + 8) * 32; }
+// An N tile wider than 128 columns is computed in two passes over the same k-blocks (columns [0, P0), then [P0, block_n)):
+// a pass keeps at most 64 accumulator registers per MMA thread. Both widths are multiples of 32 (whole ring chunks).
+__host__ __device__ constexpr int pass_n(int bn) { return bn <= 128 ? bn : (bn == 160 ? 96 : bn / 2); }
 
 struct ConvGemmParams {
   int tiles_w, tiles_h, tile_w, tile_h;
@@ -63,10 +77,8 @@ struct ConvGemmParams {
   int stream_k;              // 1: k-block granular split across CTAs, 0: whole tiles round-robin
   float* part_ws;            // [grid][2][128][BN] partial accumulators
   int* counters;             // [tiles], zero between launches
-  int seg_len;               // 3xTF32 only: k-blocks accumulated in TMEM before the RN fold into the master accumulator
+  int seg_len;               // 3xTF32 / 3xFP16: k-blocks accumulated by the tensor core before the RN fold into the master accumulator
   int b_lo_tap_off;          // 3xTF32 only: > 0: B's low parts are stored as taps [b_lo_tap_off, 2 * b_lo_tap_off) of the B tensor
-  int a_tmem;                // 3xFP16 only: 1 = the MMA warp copies every staged A tile into tensor memory (tcgen05.cp) and issues
-                             // the MMAs in the TS form (A from TMEM, only B fetched from shared memory)
   int res_split;             // 3xFP16 only: the residual tensor is in the split-fp16 format (else fp32)
   float acc_scale;           // 3xFP16 only: the accumulator is multiplied by this power of two first (weights are stored
                              // scaled by its inverse so that their low halves stay normal fp16 numbers)
@@ -76,11 +88,12 @@ template <int BN, int STAGES, int MODE = kModeTf32>
 struct SmemLayout {
   static constexpr bool SPLIT3 = MODE == kModeSplit3;
   static constexpr int kABytes = kBM * 128;
-  static constexpr int kBBytes = BN * 128;
+  static constexpr int kBBytes = pass_n(BN) * 128;     // B rows of one pass
   static constexpr int kHalf = kABytes + kBBytes;                 // bytes the two TMA loads of a k-block deliver
-  // 3xTF32: [A raw | B raw (= the hi operand: the MMA ignores the low 13 bits) | B lo]; A's hi / lo parts live in TENSOR memory
+  // 3xTF32: [A raw | B hi (masked in place by the splitters) | B lo]; the MMA warpgroups split A in registers
   static constexpr int kStageBytes = SPLIT3 ? kHalf + kBBytes : kHalf;
-  static constexpr int kEpiOffset = STAGES * kStageBytes;       // 4 warps x (2 out + 2 residual) x 4 KB
+  static constexpr int kRingOffset = STAGES * kStageBytes;
+  static constexpr int kEpiOffset = kRingOffset + kRingSlots * kRingSlotBytes;   // 4 warps x (2 out + 2 residual) x 4 KB
   static constexpr int kEpiBytes = 4 * 4 * 4096;
   static constexpr int kBarOffset = kEpiOffset + kEpiBytes;
   static constexpr int kSbCols = BN <= 128 ? 128 : 256;
@@ -153,27 +166,191 @@ struct WorkIter {
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 __device__ __forceinline__ void epi_bar_sync8() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // 8 epilogue warps
 
+// epilogue side of the accumulator ring: this thread's tile row `row`, the 32 columns of the `use`-th chunk that goes through
+// ring slot `slot`; the slot is handed back once the warp has read it (all 32 lanes call this).
+// A parity wait only tells the phase it names from its neighbours, so every warp that reads a slot must read EVERY chunk
+// of that slot, in order: then neither side can be more than one phase away from the other.
+__device__ __forceinline__ void ring_take(const uint8_t* ring, uint64_t* full, uint64_t* empty, uint32_t slot, uint32_t use,
+                                          int row, uint32_t (&r)[32]) {
+  mbar_wait(&full[slot], use & 1u);
+  const uint8_t* rowp = ring + slot * kRingSlotBytes + row * 128;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const uint4 v = *reinterpret_cast<const uint4*>(rowp + ((j ^ (row & 7)) << 4));
+    r[4 * j] = v.x; r[4 * j + 1] = v.y; r[4 * j + 2] = v.z; r[4 * j + 3] = v.w;
+  }
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[slot]);
+}
+// chunk number `seq` of a ring whose slots alternate (every reader warp of a slot reads all of its chunks)
+__device__ __forceinline__ void ring_take(const uint8_t* ring, uint64_t* full, uint64_t* empty, uint32_t seq, int row,
+                                          uint32_t (&r)[32]) {
+  ring_take(ring, full, empty, seq % kRingSlots, seq / kRingSlots, row, r);
+}
+__device__ __forceinline__ void ring_skip(const uint8_t* ring, uint64_t* full, uint64_t* empty, uint32_t slot, uint32_t use,
+                                          int row) {
+  uint32_t r[32];
+  ring_take(ring, full, empty, slot, use, row, r);
+}
+__device__ __forceinline__ void ring_skip(const uint8_t* ring, uint64_t* full, uint64_t* empty, uint32_t seq, int row) {
+  ring_skip(ring, full, empty, seq % kRingSlots, seq / kRingSlots, row);
+}
+
+// MMA side: the fragment of warpgroup-thread `wtid` (0..127) of accumulator columns [32 c, 32 c + 32) as the `use`-th chunk of
+// ring slot `slot` (rows 64 wg .. 64 wg + 63); every MMA thread arrives on the slot's full barrier
+template <int NR>
+__device__ __forceinline__ void ring_put(uint8_t* ring, uint64_t* full, uint64_t* empty, uint32_t slot, uint32_t use, int wg,
+                                         int wtid, const float (&d)[NR], const int c) {
+  if (use > 0) mbar_wait(&empty[slot], (use - 1) & 1u);
+  const int r0 = wg * 64 + (wtid >> 5) * 16 + ((wtid & 31) >> 2);
+  const int t = wtid & 3;
+  uint8_t* base = ring + slot * kRingSlotBytes;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int j = 2 * i + (t >> 1);                 // 16-byte group of columns 8 i + 2 t, + 1
+    const int off = (t & 1) * 8;
+    *reinterpret_cast<float2*>(base + r0 * 128 + ((j ^ (r0 & 7)) << 4) + off) =
+        make_float2(d[4 * (4 * c + i)], d[4 * (4 * c + i) + 1]);
+    const int r1 = r0 + 8;
+    *reinterpret_cast<float2*>(base + r1 * 128 + ((j ^ (r1 & 7)) << 4) + off) =
+        make_float2(d[4 * (4 * c + i) + 2], d[4 * (4 * c + i) + 3]);
+  }
+  mbar_arrive(&full[slot]);
+}
+
+// one k-block of MMAs of warpgroup wg: the 64 x BN slab of the tile, K = one 128-byte swizzle row
+template <int BN, int MODE>
+__device__ __forceinline__ void mma_kblock(float (&d)[BN / 2], uint32_t a_addr, uint32_t b_addr, uint32_t b_lo_addr,
+                                           const int wtid, const bool first) {
+  const uint64_t adesc = wgmma_desc_sw128(a_addr);
+  const uint64_t bdesc = wgmma_desc_sw128(b_addr);
+  if constexpr (MODE == kModeSplit3) {
+    // A from registers: hi = fp32 truncated to TF32, lo = x - hi (exact); B hi / lo from shared memory
+    // fragment of k-step k: rows g, g + 8 (g = 16 warp + lane / 4), K columns 8 k + lane % 4 and + 4
+    const int g = (wtid >> 5) * 16 + ((wtid & 31) >> 2), t = wtid & 3;
+    const uint64_t blo = wgmma_desc_sw128(b_lo_addr);
+    uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int r = g + (e & 1) * 8, col = 8 * k + t + (e >> 1) * 4;
+        float x;
+        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(a_addr + r * 128 + ((((col >> 2) ^ (r & 7)) << 4) | ((col & 3) << 2))));
+        const uint32_t h = __float_as_uint(x) & 0xffffe000u;
+        ahi[k][e] = h;
+        alo[k][e] = __float_as_uint(x - __uint_as_float(h));
+      }
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      Wgmma<BN>::tf32_rs(d, ahi[k], bdesc + 2 * k, (first && k == 0) ? 0 : 1);
+      Wgmma<BN>::tf32_rs(d, ahi[k], blo + 2 * k, 1);
+      Wgmma<BN>::tf32_rs(d, alo[k], bdesc + 2 * k, 1);
+    }
+  } else if constexpr (MODE == kModeF16x3) {
+    // a staged row = [32 hi halves | 32 lo halves] of 32 K-values: k-step j (16 values) reads hi at byte 32 j and
+    // lo at byte 64 + 32 j of the swizzle row (descriptor units of 16 bytes); hi.hi + hi.lo + lo.hi
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      Wgmma<BN>::f16_ss(d, adesc + 2 * k, bdesc + 2 * k, (first && k == 0) ? 0 : 1);
+      Wgmma<BN>::f16_ss(d, adesc + 2 * k, bdesc + 4 + 2 * k, 1);
+      Wgmma<BN>::f16_ss(d, adesc + 4 + 2 * k, bdesc + 2 * k, 1);
+    }
+  } else {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      // advance 32 B (8 floats / 16 halves) inside the swizzle row: +2 in 16-byte units
+      if (MODE == kModeF16) Wgmma<BN>::f16_ss(d, adesc + 2 * k, bdesc + 2 * k, (first && k == 0) ? 0 : 1);
+      else Wgmma<BN>::tf32_ss(d, adesc + 2 * k, bdesc + 2 * k, (first && k == 0) ? 0 : 1);
+    }
+  }
+  wgmma_commit();
+}
+
+struct MmaState {
+  int stage;
+  uint32_t phase;
+  uint32_t uses[kRingSlots];   // accumulator chunks handed to each ring slot so far
+};
+
+// The MMAs of one work item (k-blocks [kb0, kb1)) for PN columns of the tile (one pass), by MMA warpgroup wg; the result
+// goes to the ring in 32-column chunks. SPLIT3 / 3xFP16 restart the accumulator every seg_len k-blocks and fold the segments
+// into a master accumulator with round-to-nearest adds.
+// Ring slots: hpc == 0: consecutive chunks alternate over the slots (conv_gemm: every reader of a slot reads all its chunks);
+// hpc > 0: the chunk of columns [32 c, 32 c + 32) goes to slot (c / hpc) & 1, the slot of the epilogue half that finishes
+// those columns in a chain layer (hpc = 32-column chunks per epilogue chunk).
+template <int PN, int STAGES, int MODE, class L>
+__device__ __forceinline__ void mma_pass(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, uint64_t* split_bar,
+                                         uint8_t* ring, uint64_t* ring_full, uint64_t* ring_empty, MmaState& ms, int kb0,
+                                         int kb1, int seg_len, int wg, int wtid, int hpc) {
+  constexpr bool SPLIT3 = MODE == kModeSplit3;
+  constexpr bool SEG = SPLIT3 || MODE == kModeF16x3;
+  const int lane = wtid & 31;
+  float d[PN / 2];
+  float master[SEG ? PN / 2 : 1];
+  bool has_master = false;
+  for (int s0 = kb0, s1 = 0; s0 < kb1; s0 = s1) {
+    s1 = (kb1 - s0 > seg_len) ? s0 + seg_len : kb1;
+    int pending = -1;                            // stage whose MMAs may still be in flight
+    for (int kb = s0; kb < s1; ++kb) {
+      mbar_wait(SPLIT3 ? &split_bar[ms.stage] : &full_bar[ms.stage], ms.phase);
+      const uint32_t a_addr = smem_u32(smem + ms.stage * L::kStageBytes);
+      mma_kblock<PN, MODE>(d, a_addr + wg * 64 * 128, a_addr + L::kABytes, a_addr + L::kABytes + L::kBBytes, wtid, kb == s0);
+      // SPLIT3 reads its A fragments into registers for every k-block: nothing stays in flight across them
+      if (SPLIT3) wgmma_wait<0>(); else wgmma_wait<1>();
+      if (pending >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[pending]);   // frees the smem slot: its MMAs have retired
+      }
+      pending = ms.stage;
+      if (++ms.stage == STAGES) {
+        ms.stage = 0;
+        ms.phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_wait_regs(d);
+    if (pending >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[pending]);
+    }
+    if constexpr (SEG) {
+#pragma unroll
+      for (int i = 0; i < PN / 2; ++i) master[i] = has_master ? __fadd_rn(d[i], master[i]) : d[i];
+      has_master = true;
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < PN / 32; ++c) {
+    uint32_t slot;
+    if (hpc == 0) slot = (ms.uses[0] == ms.uses[1]) ? 0u : 1u;    // alternate
+    else slot = static_cast<uint32_t>((c / hpc) & 1);
+    const uint32_t use = ms.uses[slot]++;
+    if constexpr (SEG) ring_put(ring, ring_full, ring_empty, slot, use, wg, wtid, master, c);
+    else ring_put(ring, ring_full, ring_empty, slot, use, wg, wtid, d, c);
+  }
+}
+
 // Persistent stream-K kernel. The work is the list of (tile, k-block) units, tiles ordered
 // (batch, n-tile, m-tile) with m fastest; CTA c owns the contiguous unit range
 // [c*U/G, (c+1)*U/G). A tile whose k-blocks straddle CTAs is finished by the last CTA to
 // arrive, which sums the partial accumulators (in CTA order -> deterministic) and runs the
-// epilogue. Accumulators are double-buffered in TMEM so the epilogue of item i overlaps the
-// MMAs of item i+1.
-// SPLIT3 ("3xTF32"): operands arrive as full fp32; four extra warps split every staged tile into hi = fp32 truncated to
-// TF32 and lo = x - hi (exact), and each k-step issues hi*hi + hi*lo + lo*hi into the same accumulator: ~2^-19 relative
-// error instead of 2^-11, for the strict-parity mode. Round 1 kept all four split tiles in shared memory (224 KB of smem
-// traffic per 128 x 128 x 32 k-block: TMA 32 + split 96 + twelve MMAs reading both operands 96), which bound the mode at
-// ~100 TFLOP/s. Now the A operand is a TENSOR-MEMORY operand (tcgen05.mma "TS" form): a splitter thread reads its row of
-// the raw A tile once (8 x LDS.128) and writes hi / lo straight into two 32-column TMEM slabs with tcgen05.st; the MMAs
-// read A from TMEM and only B (the raw tile as hi, lo beside it) from shared memory: 128 KB per k-block, and the stage shrinks
-// from 64 to 48 KB (3 stages instead of 2 at block_n 128).
+// epilogue. The MMA warpgroups compute item i+1 in registers while the epilogue warps finish
+// item i from the accumulator ring.
+// SPLIT3 ("3xTF32"): operands arrive as full fp32; four splitter warps rewrite every staged B tile as hi = fp32 truncated
+// to TF32 (in place) and lo = x - hi (behind it), the MMA warpgroups split their A fragments the same way in registers, and
+// each k-step issues hi*hi + hi*lo + lo*hi into the same accumulator: ~2^-19 relative error instead of 2^-11, for the
+// strict-parity mode.
 // OUT16: output (and residual) tensors are fp16; the epilogue then works in chunks of 64 columns (= one 128-byte
 // swizzle row of halves) instead of 32.
-// Programmatic dependent launch: the prologue (barrier init, TMEM allocation, descriptor prefetch) runs before
-// griddepcontrol.wait, i.e. overlapped with the tail of the previous kernel on the stream; nothing before the wait
-// touches global memory.
+// Programmatic dependent launch: the prologue (barrier init, descriptor prefetch) runs before griddepcontrol.wait, i.e.
+// overlapped with the tail of the previous kernel on the stream; nothing before the wait touches global memory.
 template <int BN, int STAGES, int MODE, bool OUT16>
-__global__ void __launch_bounds__(kThreads + ((MODE == kModeSplit3 || MODE == kModeF16x3) ? 128 : 0), 1)
+__global__ void __launch_bounds__(conv_gemm_threads(MODE), 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes,
                       const ConvGemmParams p) {
@@ -183,25 +360,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr bool OUTH = OUT16 && !PK;           // plain fp16 output
   constexpr int kBK = mode_bk(MODE);
   constexpr int CW = OUTH ? 64 : 32;   // epilogue chunk: columns per 128-byte output row segment
+  constexpr int kMmaWarp0 = mma_warp0(MODE);
   static_assert(!OUTH || BN % 64 == 0, "fp16 output needs block_n % 64 == 0");
   static_assert(SmemLayout<BN, STAGES, MODE>::kTotal <= 227 * 1024, "pipeline + staging exceed the 227 KB of a CTA");
   using L = SmemLayout<BN, STAGES, MODE>;
-  // accumulators: two ping-pong buffers (+ a master accumulator in 3xTF32 mode, see kSegLen)
-  // 3xFP16: eight epilogue warps, the master accumulator in their REGISTERS (64 columns per thread), see the epilogue below
-  constexpr bool REGM = PK;
-  constexpr uint32_t kAccBufs = (SEG && !REGM) ? 3 : 2;
-  // 3xTF32: three accumulators + two A slabs of 64 columns (hi: 32 columns of K, lo: the next 32)
-  constexpr uint32_t kNeedCols = kAccBufs * BN + (SPLIT3 ? 128 : 0) + (PK ? 64 : 0);   // 3xFP16: two 32-column A slabs
-  static_assert(kNeedCols <= 512, "accumulators + A slabs exceed the 512 TMEM columns");
-  constexpr uint32_t kTmemCols = (kNeedCols <= 64) ? 64 : (kNeedCols <= 128) ? 128 : (kNeedCols <= 256) ? 256 : 512;
-  constexpr uint32_t kAccStride = (SEG && !REGM) ? BN : kTmemCols / 2;
-  constexpr uint32_t kASlab = 3 * BN;        // first column of A slab 0 (3xTF32); slab s at + 64 s
-  constexpr uint32_t kASlabPk = kTmemCols - 64;   // 3xFP16 (a_tmem): slab s = 32 columns at + 32 s: [hi k0 | hi k1 | lo k0 | lo k1] x 8
   // The tensor core adds into its fp32 accumulator with truncation, a bias that grows with the length of the
-  // accumulation chain (measured ~1e-3 relative after 3000 k-blocks; ~2e-5 after 32, which the chaotic position
-  // embedding of the relation module amplifies to 5e-3 on the final logits). The strict mode therefore restarts the
-  // TMEM accumulator every kSegLen k-blocks (4 k-blocks = 48 truncating adds, <= 3e-6 relative) and folds the segments into a master accumulator (also in TMEM)
-  // with round-to-nearest fp32 adds done by the epilogue warps.
+  // accumulation chain (~2e-5 relative after 32 k-blocks, which the chaotic position embedding of the relation module
+  // amplifies to 5e-3 on the final logits). The strict modes therefore restart the accumulator every kSegLen k-blocks
+  // and fold the segments into a master accumulator (registers of the MMA warpgroups) with round-to-nearest fp32 adds.
   const int kSegLen = SEG ? p.seg_len : 0x7fffffff;   // k-blocks per accumulator segment (mega_set_split3_seg_len, default 4)
   extern __shared__ uint8_t smem_raw[];
   // the 128B swizzle pattern is a function of the absolute smem address: align to 1024 B
@@ -210,12 +376,11 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* split_bar = empty_bar + STAGES;       // [STAGES] (3xTF32 only)
-  uint64_t* tmem_full_bar = split_bar + STAGES;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;   // [2]
-  uint64_t* res_bar = tmem_empty_bar + 2;         // [4 warps][2] (3xFP16: [8 warps][2])
-  uint64_t* aslab_empty_bar = res_bar + 16;        // [2] (3xTF32: the MMAs that read A slab s have completed)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(aslab_empty_bar + 2);
-  int* epi_flag = reinterpret_cast<int*>(tmem_slot + 1);
+  uint64_t* ring_full = split_bar + STAGES;       // [kRingSlots]
+  uint64_t* ring_empty = ring_full + kRingSlots;  // [kRingSlots]
+  uint64_t* res_bar = ring_empty + kRingSlots;    // [4 warps][2] (3xFP16: [8 warps][2])
+  int* epi_flag = reinterpret_cast<int*>(res_bar + 16);
+  uint8_t* ring = smem + L::kRingOffset;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -233,27 +398,19 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);      // one arrival per MMA warp
       mbar_init(&split_bar[s], 4);
     }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full_bar[b], 1);
-      mbar_init(&tmem_empty_bar[b], PK ? 8 : 4);
+    for (int b = 0; b < kRingSlots; ++b) {
+      mbar_init(&ring_full[b], 256);    // every MMA thread
+      mbar_init(&ring_empty[b], 4);     // the four epilogue warps that read a slot
     }
     for (int b = 0; b < 16; ++b) mbar_init(&res_bar[b], 1);
-    for (int b = 0; b < 2; ++b) mbar_init(&aslab_empty_bar[b], 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, kTmemCols);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_wait();               // the previous kernel's results (and its reads of our outputs) are complete
   griddep_launch_dependents();  // let the next kernel's prologue overlap this kernel
-
   if (warp == 0) {
     // ===================== TMA producer =====================
     // lane 0 loads the A (activation) tile and posts the expected byte count, lane 1 the B (weight) tile, so the two
@@ -266,13 +423,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       int kb0, kb1;
       const int k_chunks = p.k_chunks, taps_s = p.taps_s;
       while (it.next(t, kb0, kb1)) {
-        const TileCoord tc = decode_tile(p, t, BN);
+       const TileCoord tc = decode_tile(p, t, BN);
+       for (int pass = 0; pass < (BN > pass_n(BN) ? 2 : 1); ++pass) {
         int tap = kb0 / k_chunks;
         int kc = kb0 - tap * k_chunks;
         int r = tap / taps_s;
         int sx = tap - r * taps_s;
         const int a_c0 = tc.batch * p.a_c_off, a_n = tc.img + tc.batch * p.a_n_off;
-        const int b_k0 = tc.batch * p.b_k_off, b_n = tc.n0 + tc.batch * p.b_n_off;
+        const int b_k0 = tc.batch * p.b_k_off, b_n = tc.n0 + pass * pass_n(BN) + tc.batch * p.b_n_off;
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* a_dst = smem + stage * L::kStageBytes;
@@ -299,149 +457,54 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             phase ^= 1;
           }
         }
+       }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = (MODE == kModeF16 || PK) ? umma_idesc<0>(kBM, BN) : umma_idesc<2>(kBM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      WorkIter it(p, cta, grid);
-      int t;
-      int kb0, kb1;
-      int item = 0;
-      uint32_t kbn = 0;            // k-blocks issued by this CTA (3xTF32: A slab = kbn & 1)
-      while (it.next(t, kb0, kb1)) {
-        for (int s0 = kb0, s1 = 0; s0 < kb1; s0 = s1, ++item) {
-          s1 = (kb1 - s0 > kSegLen) ? s0 + kSegLen : kb1;
-          const int buf = item & 1;
-          const uint32_t use = static_cast<uint32_t>(item >> 1);
-          mbar_wait(&tmem_empty_bar[buf], (use & 1) ^ 1);   // epilogue drained this accumulator
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + buf * kAccStride;
-          for (int kb = s0; kb < s1; ++kb, ++kbn) {
-            mbar_wait(SPLIT3 ? &split_bar[stage] : &full_bar[stage], phase);
-            tc_fence_after();
-            const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
-            const uint32_t b_addr = a_addr + L::kABytes;
-            const uint64_t adesc = umma_desc_sw128(a_addr);
-            const uint64_t bdesc = umma_desc_sw128(b_addr);
-            if (SPLIT3) {
-              // A from tensor memory: slab (kbn & 1), hi in its columns [0, 32), lo in [32, 64); 8 columns of K per MMA
-              const uint32_t a_hi = tmem_base + kASlab + (kbn & 1u) * 64u, a_lo = a_hi + 32u;
-              const uint64_t blo = umma_desc_sw128(b_addr + L::kBBytes);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                umma_tf32_ts(tmem_d, a_hi + 8 * k, bdesc + 2 * k, idesc, (kb > s0 || k > 0) ? 1u : 0u);
-                umma_tf32_ts(tmem_d, a_hi + 8 * k, blo + 2 * k, idesc, 1u);
-                umma_tf32_ts(tmem_d, a_lo + 8 * k, bdesc + 2 * k, idesc, 1u);
-              }
-              umma_commit(&aslab_empty_bar[kbn & 1u]);   // the splitter may overwrite this A slab
-            } else if (PK && p.a_tmem) {
-              // TS form: the four 128 x 32-byte slices of the A tile (hi / lo of the two k-steps) go to a tensor-memory slab by
-              // tcgen05.cp (same descriptors the SS-form MMAs would read them through; cp and mma issued by one thread
-              // execute in order), then the MMAs fetch only B from shared memory: 24 KB of operand reads per k-block
-              // instead of 48 KB (+ 16 KB read once by the copies)
-              const uint32_t a_tm = tmem_base + kASlabPk + (kbn & 1u) * 32u;
-#pragma unroll
-              for (int c = 0; c < 4; ++c) tmem_cp_128x256b(a_tm + 8 * c, adesc + 2 * c);
-#pragma unroll
-              for (int k = 0; k < 2; ++k) {
-                umma_f16_ts(tmem_d, a_tm + 8 * k, bdesc + 2 * k, idesc, (kb > s0 || k > 0) ? 1u : 0u);
-                umma_f16_ts(tmem_d, a_tm + 8 * k, bdesc + 4 + 2 * k, idesc, 1u);
-                umma_f16_ts(tmem_d, a_tm + 16 + 8 * k, bdesc + 2 * k, idesc, 1u);
-              }
-            } else if (PK) {
-              // a staged row = [32 hi halves | 32 lo halves] of 32 K-values: k-step j (16 values) reads hi at byte 32 j and
-              // lo at byte 64 + 32 j of the swizzle row (descriptor units of 16 bytes); hi.hi + hi.lo + lo.hi
-#pragma unroll
-              for (int k = 0; k < 2; ++k) {
-                umma_f16(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > s0 || k > 0) ? 1u : 0u);
-                umma_f16(tmem_d, adesc + 2 * k, bdesc + 4 + 2 * k, idesc, 1u);
-                umma_f16(tmem_d, adesc + 4 + 2 * k, bdesc + 2 * k, idesc, 1u);
-              }
-            } else {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                // advance 32 B (8 floats / 16 halves) inside the swizzle row: +2 in 16-byte units
-                if (MODE == kModeF16) {
-                  umma_f16(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > s0 || k > 0) ? 1u : 0u);
-                } else {
-                  umma_tf32(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > s0 || k > 0) ? 1u : 0u);
-                }
-              }
-            }
-            umma_commit(&empty_bar[stage]);  // frees the smem slot once these MMAs retire
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
-          umma_commit(&tmem_full_bar[buf]);
-        }
-      }
+  } else if (warp >= kMmaWarp0) {
+    // ===================== MMA warpgroups =====================
+    const int wg = (warp - kMmaWarp0) >> 2;          // tile rows [64 wg, 64 wg + 64)
+    const int wtid = threadIdx.x - (kMmaWarp0 + 4 * wg) * 32;
+    constexpr int P0 = pass_n(BN), P1 = BN - P0;
+    MmaState ms = {0, 0, {0, 0}};
+    WorkIter it(p, cta, grid);
+    int t;
+    int kb0, kb1;
+    while (it.next(t, kb0, kb1)) {
+      mma_pass<P0, STAGES, MODE, L>(smem, full_bar, empty_bar, split_bar, ring, ring_full, ring_empty, ms, kb0, kb1, kSegLen,
+                                    wg, wtid, 0);
+      if constexpr (P1 > 0)
+        mma_pass<P1, STAGES, MODE, L>(smem, full_bar, empty_bar, split_bar, ring, ring_full, ring_empty, ms, kb0, kb1,
+                                      kSegLen, wg, wtid, 0);
     }
-  } else if (warp >= 6 && !PK) {
+  } else if (warp >= 6 && warp < 10 && !PK) {
     // ===================== operand splitter (3xTF32 only, warps 6..9) =====================
+    // B: hi = x truncated to TF32 written back in place, lo = x - hi into the region behind the raw tile (pre-split weights
+    // bring lo by TMA: only the hi mask is applied). A is split by the MMA warpgroups while they load their fragments.
     if (SPLIT3) {
       const int stid = threadIdx.x - kThreads;            // 0..127
-      const int arow = (warp & 3) * 32 + lane;            // the A-tile row = TMEM lane this thread may write
-      const uint32_t lane_bits = static_cast<uint32_t>((warp & 3) * 32) << 16;
       int stage = 0;
       uint32_t phase = 0;
-      uint32_t kbn = 0;
       WorkIter it(p, cta, grid);
       int t;
       int kb0, kb1;
+      const bool need_lo = p.b_lo_tap_off == 0;
       while (it.next(t, kb0, kb1)) {
-        for (int kb = kb0; kb < kb1; ++kb, ++kbn) {
+        for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&full_bar[stage], phase);
-          uint8_t* base = smem + stage * L::kStageBytes;
-          // ---- A: this thread's row (32 floats = 128 bytes, 16-byte chunks swizzled by row & 7) -> hi / lo -> TMEM
-          {
-            const uint8_t* rowp = base + arow * 128;
-            uint32_t hi[32], lo[32];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 x = *reinterpret_cast<const float4*>(rowp + ((j ^ (arow & 7)) << 4));
-              const float xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const uint32_t h = __float_as_uint(xs[e]) & 0xffffe000u;
-                hi[4 * j + e] = h;
-                lo[4 * j + e] = __float_as_uint(xs[e] - __uint_as_float(h));
-              }
-            }
-            const uint32_t slab = kbn & 1u;
-            // the MMAs of k-block kbn - 2 (the previous user of this slab) have completed
-            if (kbn >= 2) mbar_wait(&aslab_empty_bar[slab], ((kbn >> 1) - 1) & 1u);
-            tc_fence_after();
-            const uint32_t ta = tmem_base + kASlab + slab * 64u + lane_bits;
-            __syncwarp();
-            tmem_st_32x32(ta, hi);
-            tmem_st_32x32(ta + 32u, lo);
-          }
-          // ---- B: lo = x - trunc_tf32(x) into the region behind the raw tile. The raw tile itself serves as the hi
-          //      operand: kind::tf32 reads the upper 19 bits of a 32-bit container and IGNORES the low 13 mantissa bits
-          //      (truncation, not rounding -- measured with tools/tf32_trunc_probe.py: (1 + 0.75 * 2^-10) * 1 = 1.0 on
-          //      both operand sides), so writing the masked copy back would only cost shared-memory bandwidth
-          if (p.b_lo_tap_off == 0) {      // (pre-split weights: the producer fetched lo by TMA, nothing to do for B)
-            uint8_t* bb = base + L::kABytes;
-            constexpr int kVecs = L::kBBytes / 16;
+          uint8_t* bb = smem + stage * L::kStageBytes + L::kABytes;
+          constexpr int kVecs = L::kBBytes / 16;
 #pragma unroll 4
-            for (int v = stid; v < kVecs; v += 128) {
-              const float4 x = *reinterpret_cast<const float4*>(bb + v * 16);
-              float4 l;
-              l.x = x.x - __uint_as_float(__float_as_uint(x.x) & 0xffffe000u);
-              l.y = x.y - __uint_as_float(__float_as_uint(x.y) & 0xffffe000u);
-              l.z = x.z - __uint_as_float(__float_as_uint(x.z) & 0xffffe000u);
-              l.w = x.w - __uint_as_float(__float_as_uint(x.w) & 0xffffe000u);
-              *reinterpret_cast<float4*>(bb + L::kBBytes + v * 16) = l;
-            }
+          for (int v = stid; v < kVecs; v += 128) {
+            float4 x = *reinterpret_cast<const float4*>(bb + v * 16);
+            float4 h;
+            h.x = __uint_as_float(__float_as_uint(x.x) & 0xffffe000u);
+            h.y = __uint_as_float(__float_as_uint(x.y) & 0xffffe000u);
+            h.z = __uint_as_float(__float_as_uint(x.z) & 0xffffe000u);
+            h.w = __uint_as_float(__float_as_uint(x.w) & 0xffffe000u);
+            *reinterpret_cast<float4*>(bb + v * 16) = h;
+            if (need_lo)
+              *reinterpret_cast<float4*>(bb + L::kBBytes + v * 16) = make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
           }
-          tmem_st_wait();
-          tc_fence_before();
           fence_async_smem();
           __syncwarp();
           if (lane == 0) mbar_arrive(&split_bar[stage]);
@@ -452,19 +515,16 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if constexpr (PK) {
+  } else if (warp >= 2 && warp < 10 && PK) {
     // ===================== epilogue, 3xFP16 (warps 2..9) =====================
-    // Two warps share a TMEM lane quarter (32 tile rows); each owns HALF of the tile's columns: kCPW chunks of 32. What
-    // the 4-warp epilogue above measured on this mode (10-13 us per 128 x 128 tile at K = 256 against 2.7 us of MMAs) came
-    // from (i) the RN folds -- segment + master read from tensor memory (64 B/cycle per SM) and written back, 0.85-1.2 us
-    // each: here the master lives in REGISTERS (64 columns per thread) and a fold reads the segment once; (ii) two
-    // CTA-wide barriers around L1-missing scale / bias loads per tile: here the BN scale is folded into the packed
-    // weights, the bias slice of the NEXT tile is fetched during the current one (double-buffered, one barrier per tile);
-    // (iii) separate residual staging: here the residual lands in the store staging buffer itself (every thread reads its
-    // 128-byte row into registers before it writes the same row), issued for both chunks at the start of the tile.
+    // Two warps share a 32-row quarter of the tile; of its 32-column chunks each takes every other one (chunk cj = 2 j + half):
+    // every ring slot is read by the four warps of one half. The BN scale is folded into the packed weights, the bias slice
+    // of the NEXT tile is fetched during the current one (double-buffered, one barrier per tile), and the residual lands in
+    // the store staging buffer itself (every thread reads its 128-byte row into registers before it writes the same row),
+    // issued for all chunks at the start of the tile.
     constexpr int kCPW = BN / 64;          // 32-column chunks per warp
-    const int q = warp & 3;                // TMEM lane quarter this warp may read
-    const int half = (warp - 2) >> 2;      // which half of the columns
+    const int q = warp & 3;                // 32-row quarter of the tile
+    const int half = (warp - 2) >> 2;      // which of the interleaved chunks
     const int row = q * 32 + lane;
     const int epi_tid = (warp - 2) * 32 + lane;                              // 0 .. 255
     uint8_t* stage_buf = smem + L::kEpiOffset + (warp - 2) * (kCPW * 4096);  // kCPW x 4 KB: residual in, result out
@@ -474,43 +534,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     WorkIter it(p, cta, grid);
     int t;
     int kb0, kb1;
-    int item = 0;
-    const uint32_t lane_bits = static_cast<uint32_t>(q * 32) << 16;
-    const uint32_t col_base = static_cast<uint32_t>(half * kCPW * 32);
+    uint32_t seq0 = 0;    // ring chunk number of this item's column 0
     const uint32_t sw = static_cast<uint32_t>(lane & 7);
     const bool res_split = p.res_split != 0;
     const float slope = p.relu == 2 ? 0.1f : 0.f;
-    float master[kCPW * 32];
-    for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item) {
+    for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item, seq0 += BN / 32) {
       const TileCoord tc = decode_tile(p, t, BN);
-      // ---- fold every segment but the last into the register master (round-to-nearest fp32 adds)
-      bool has_master = false;
-      int s0 = kb0;
-      for (; s0 + kSegLen < kb1; s0 += kSegLen, ++item) {
-        const int fb = item & 1;
-        mbar_wait(&tmem_full_bar[fb], static_cast<uint32_t>(item >> 1) & 1);
-        tc_fence_after();
-        const uint32_t seg_row = tmem_base + fb * kAccStride + lane_bits + col_base;
-#pragma unroll
-        for (int j = 0; j < kCPW; ++j) {
-          uint32_t a[32];
-          __syncwarp();
-          tmem_ld_32x32(seg_row + j * 32, a);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float v = __uint_as_float(a[i]);
-            master[j * 32 + i] = has_master ? __fadd_rn(v, master[j * 32 + i]) : v;
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty_bar[fb]);
-        has_master = true;
-      }
-      const int buf = item & 1;
-      const uint32_t use = static_cast<uint32_t>(item >> 1);
-      ++item;
       const bool complete = (kb0 == 0 && kb1 == KB);
       const int r0 = q * 32;
       const int bh0 = r0 / p.tile_w, bw0 = r0 - bh0 * p.tile_w;
@@ -546,7 +575,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (p.has_residual && lane == 0) {
 #pragma unroll
           for (int j = 0; j < kCPW; ++j) {
-            const int cj = half * kCPW + j;
+            const int cj = 2 * j + half;
             if (cj < nchunks) {
               mbar_arrive_expect_tx(&rbar[j], 4096);
               tma_load_4d(stage_buf + j * 4096, &tmRes, &rbar[j], tc.n0 + cj * 32 + tc.batch * p.res_c_off, st_w, st_h, res_n);
@@ -555,39 +584,24 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       };
       if (complete) issue_residual();
-      mbar_wait(&tmem_full_bar[buf], use & 1);
-      tc_fence_after();
-      const uint32_t tmem_row = tmem_base + buf * kAccStride + lane_bits + col_base;
-      // chunk j of my columns: last segment (+ master). One chunk is live at a time (168 registers per thread at 320 threads)
       auto load_chunk = [&](const int j, float (&acc)[32]) {
         uint32_t raw[32];
-        __syncwarp();
-        tmem_ld_32x32(tmem_row + j * 32, raw);
-        tmem_ld_wait();
+        ring_take(ring, ring_full, ring_empty, seq0 + 2 * j + half, row, raw);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const float v = __uint_as_float(raw[i]);
-          acc[i] = has_master ? __fadd_rn(v, master[j * 32 + i]) : v;
-        }
-      };
-      const int my_chunks = max(0, min(kCPW, nchunks - half * kCPW));
-      auto release_acc = [&]() {      // hand the accumulator buffer back to the MMA warp
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty_bar[buf]);
+        for (int i = 0; i < 32; ++i) acc[i] = __uint_as_float(raw[i]);
       };
       bool finalize = complete;
       int c_first = cta, c_last = cta;
       if (!complete) {
-        // ---- publish this CTA's partial accumulator (my columns), then find out whether it arrived last
-        float* my_ws = p.part_ws + ((static_cast<long long>(cta) * 2 + (tile_item == 0 ? 0 : 1)) * kBM + row) * BN + col_base;
+        // ---- publish this CTA's partial accumulator (my chunks), then find out whether it arrived last
+        float* my_ws = p.part_ws + ((static_cast<long long>(cta) * 2 + (tile_item == 0 ? 0 : 1)) * kBM + row) * BN;
 #pragma unroll
         for (int j = 0; j < kCPW; ++j) {
           float acc[32];
           load_chunk(j, acc);
 #pragma unroll
           for (int i = 0; i < 32; i += 4)
-            __stcg(reinterpret_cast<float4*>(my_ws + j * 32 + i), make_float4(acc[i], acc[i + 1], acc[i + 2], acc[i + 3]));
+            __stcg(reinterpret_cast<float4*>(my_ws + (2 * j + half) * 32 + i), make_float4(acc[i], acc[i + 1], acc[i + 2], acc[i + 3]));
         }
         __threadfence();
         epi_bar_sync8();
@@ -607,37 +621,28 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           issue_residual();
         }
       }
-      if (!finalize || my_chunks == 0) release_acc();
       if (finalize) {
         const int out_n = tc.img + tc.batch * p.out_n_off;
 #pragma unroll
         for (int j = 0; j < kCPW; ++j) {
-          if (j < my_chunks) {
-            const int cj = half * kCPW + j;
+          const int cj = 2 * j + half;
+          if (cj < nchunks) {
             float acc[32];
-            load_chunk(j, acc);
-            if (j + 1 == my_chunks) release_acc();
-            if (!complete) {
-              // deterministic reduction: parts summed in CTA order, own part from tensor memory
-              float sum[32];
+            if (complete) {
+              load_chunk(j, acc);
+            } else {
+              // deterministic reduction: parts summed in CTA order (this CTA's own part as published above)
 #pragma unroll
-              for (int i = 0; i < 32; ++i) sum[i] = 0.f;
+              for (int i = 0; i < 32; ++i) acc[i] = 0.f;
               for (int oc = c_first; oc <= c_last; ++oc) {
-                if (oc == cta) {
+                const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
+                const float* ws = p.part_ws + ((static_cast<long long>(oc) * 2 + slot) * kBM + row) * BN + cj * 32;
 #pragma unroll
-                  for (int i = 0; i < 32; ++i) sum[i] += acc[i];
-                } else {
-                  const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
-                  const float* ws = p.part_ws + ((static_cast<long long>(oc) * 2 + slot) * kBM + row) * BN + col_base + j * 32;
-#pragma unroll
-                  for (int i = 0; i < 32; i += 4) {
-                    const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + i));
-                    sum[i] += v.x; sum[i + 1] += v.y; sum[i + 2] += v.z; sum[i + 3] += v.w;
-                  }
+                for (int i = 0; i < 32; i += 4) {
+                  const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + i));
+                  acc[i] += v.x; acc[i + 1] += v.y; acc[i + 2] += v.z; acc[i + 3] += v.w;
                 }
               }
-#pragma unroll
-              for (int i = 0; i < 32; ++i) acc[i] = sum[i];
             }
             uint8_t* rowp = stage_buf + j * 4096 + lane * 128;
             const float4* biv = reinterpret_cast<const float4*>(bias_s + bsel * BN + cj * 32);
@@ -701,15 +706,17 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               tma_store_4d(&tmOut, stage_buf + j * 4096, tc.n0 + cj * 32 + tc.batch * p.out_c_off, st_w, st_h, out_n);
               tma_store_commit();
             }
+          } else if (complete) {
+            ring_skip(ring, ring_full, ring_empty, seq0 + cj, row);   // columns past cout: hand the slot back unread
           }
         }
       }
       if (has_next && epi_tid < BN) bias_s[(bsel ^ 1) * BN + epi_tid] = next_bias;
     }
     if (lane == 0) tma_store_wait<0>();   // global writes complete before the CTA retires
-  } else {
+  } else if (warp >= 2 && warp < 6) {
     // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;  // TMEM lane quarter this warp may read
+    const int q = warp & 3;  // 32-row quarter of the tile
     const int row = q * 32 + lane;
     const int epi_tid = (warp - 2) * 32 + lane;
     uint8_t* epi_out = smem + L::kEpiOffset + (warp - 2) * 16384;   // 2 x 4 KB store staging
@@ -720,43 +727,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     WorkIter it(p, cta, grid);
     int t;
     int kb0, kb1;
-    int item = 0;   // accumulator-segment counter (ping-pong bookkeeping shared with the MMA warp)
-    const uint32_t lane_bits = static_cast<uint32_t>(q * 32) << 16;
-    const uint32_t master_row = tmem_base + 2 * kAccStride + lane_bits;
-    for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item) {
+    uint32_t seq0 = 0;    // ring chunk number of this item's column 0
+    for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item, seq0 += BN / 32) {
       const TileCoord tc = decode_tile(p, t, BN);
-      // ---- 3xTF32 only: fold every segment but the last into the master accumulator (RN fp32 adds)
-      bool has_master = false;
-      int s0 = kb0;
-      for (; SEG && s0 + kSegLen < kb1; s0 += kSegLen, ++item) {
-        const int fb = item & 1;
-        mbar_wait(&tmem_full_bar[fb], static_cast<uint32_t>(item >> 1) & 1);
-        tc_fence_after();
-        const uint32_t seg_row = tmem_base + fb * kAccStride + lane_bits;
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          uint32_t a[32];
-          __syncwarp();
-          tmem_ld_32x32(seg_row + c * 32, a);
-          tmem_ld_wait();
-          if (has_master) {
-            uint32_t m[32];
-            tmem_ld_32x32(master_row + c * 32, m);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) a[j] = __float_as_uint(__fadd_rn(__uint_as_float(a[j]), __uint_as_float(m[j])));
-          }
-          tmem_st_32x32(master_row + c * 32, a);
-        }
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty_bar[fb]);
-        has_master = true;
-      }
-      const int buf = item & 1;
-      const uint32_t use = static_cast<uint32_t>(item >> 1);
-      ++item;
       const bool complete = (kb0 == 0 && kb1 == KB);
       // ---- while the MMAs of this tile run: stage its scale / bias slice in shared memory (the chunk loop then reads
       //      them with broadcast LDS instead of L1-missing global loads) and start the first residual load
@@ -777,22 +750,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         tma_load_4d(epi_res, &tmRes, &rbar[0], tc.n0 + tc.batch * p.res_c_off, st_w, st_h, res_n);
       }
       epi_bar_sync();
-      mbar_wait(&tmem_full_bar[buf], use & 1);
-      tc_fence_after();
-      const uint32_t tmem_row = tmem_base + buf * kAccStride + lane_bits;
-      // accumulator chunk c (32 columns of this thread's row): last segment (+ master)
-      auto load_acc = [&](int c, uint32_t (&acc)[32]) {
-        __syncwarp();  // tcgen05.ld is .sync.aligned
-        tmem_ld_32x32(tmem_row + c * 32, acc);
-        tmem_ld_wait();
-        if (SEG && has_master) {
-          uint32_t m[32];
-          tmem_ld_32x32(master_row + c * 32, m);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = __float_as_uint(__fadd_rn(__uint_as_float(acc[j]), __uint_as_float(m[j])));
-        }
-      };
       bool finalize = complete;
       int c_first = cta, c_last = cta;
       if (!complete) {
@@ -800,7 +757,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         float* my_ws = p.part_ws + ((static_cast<long long>(cta) * 2 + (tile_item == 0 ? 0 : 1)) * kBM + row) * BN;
         auto publish = [&](const int c) {
           uint32_t acc[32];
-          load_acc(c, acc);
+          ring_take(ring, ring_full, ring_empty, seq0 + c, row, acc);
 #pragma unroll
           for (int j = 0; j < 32; j += 4) {
             float4 v = make_float4(__uint_as_float(acc[j]), __uint_as_float(acc[j + 1]),
@@ -857,33 +814,26 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           // 32 accumulator columns at a time (keeps the live registers at 32 + a handful: the 64-wide form spilled)
         #pragma unroll
           for (int h = 0; h < CW / 32; ++h) {
-            uint32_t raw[32];
-            load_acc(c * (CW / 32) + h, raw);
-            float acc[32];
-        #pragma unroll
-            for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(raw[j]);
             const int col0 = c * CW + h * 32;     // first column of this half inside the tile
-            if (!complete) {
-              // deterministic reduction: parts summed in CTA order, own part from TMEM
-              float sum[32];
+            float acc[32];
+            if (complete) {
+              uint32_t raw[32];
+              ring_take(ring, ring_full, ring_empty, seq0 + col0 / 32, row, raw);
         #pragma unroll
-              for (int j = 0; j < 32; ++j) sum[j] = 0.f;
+              for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(raw[j]);
+            } else {
+              // deterministic reduction: parts summed in CTA order (this CTA's own part as published above)
+        #pragma unroll
+              for (int j = 0; j < 32; ++j) acc[j] = 0.f;
               for (int oc = c_first; oc <= c_last; ++oc) {
-                if (oc == cta) {
+                const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
+                const float* ws = p.part_ws + ((static_cast<long long>(oc) * 2 + slot) * kBM + row) * BN + col0;
         #pragma unroll
-                  for (int j = 0; j < 32; ++j) sum[j] += acc[j];
-                } else {
-                  const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
-                  const float* ws = p.part_ws + ((static_cast<long long>(oc) * 2 + slot) * kBM + row) * BN + col0;
-        #pragma unroll
-                  for (int j = 0; j < 32; j += 4) {
-                    const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + j));
-                    sum[j] += v.x; sum[j + 1] += v.y; sum[j + 2] += v.z; sum[j + 3] += v.w;
-                  }
+                for (int j = 0; j < 32; j += 4) {
+                  const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + j));
+                  acc[j] += v.x; acc[j + 1] += v.y; acc[j + 2] += v.z; acc[j + 3] += v.w;
                 }
               }
-        #pragma unroll
-              for (int j = 0; j < 32; ++j) acc[j] = sum[j];
             }
             if (has_sb) {
               const float4* scv = reinterpret_cast<const float4*>(sb_s + col0);
@@ -946,19 +896,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll 1
         for (int c = 0; c < nchunks; ++c) finish_chunk(c);
       }
-      // release the accumulator buffer to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty_bar[buf]);
+      if (complete) {
+        // columns past cout: hand their ring slots back unread
+#pragma unroll 1
+        for (int c = nchunks * (CW / 32); c < BN / 32; ++c) ring_skip(ring, ring_full, ring_empty, seq0 + c, row);
+      }
     }
     if (lane == 0) tma_store_wait<0>();   // global writes complete before the CTA retires
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
@@ -977,7 +921,7 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUte
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
-  cfg.blockDim = dim3(kThreads + ((MODE == kModeSplit3 || MODE == kModeF16x3) ? 128 : 0), 1, 1);
+  cfg.blockDim = dim3(conv_gemm_threads(MODE), 1, 1);
   cfg.dynamicSmemBytes = L::kTotal;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];

@@ -1,6 +1,6 @@
 // Memory-bound helpers of the backbone and the window/memory plumbing:
 //   * stem im2col (7x7 / stride 2 / pad 3 over the NCHW input image -> K-major GEMM operand),
-//     feeding the tcgen05 GEMM for BaseStem.conv1 (modeling/backbone/resnet.py:347-366);
+//     feeding the wgmma GEMM for BaseStem.conv1 (modeling/backbone/resnet.py:347-366);
 //   * 3x3 / stride 2 / pad 1 max-pool in NHWC (resnet.py:365);
 //   * row gather (replaces the torch.cat of 25-deep deques every frame,
 //     detector/generalized_rcnn_mega.py:213-216 and roi_box_feature_extractors.py:674-688);
@@ -249,7 +249,7 @@ __global__ void copy_rows_batch_kernel(const __grid_constant__ CopyJobs jobs) {
 
 static int grid_for(long long total, int block) {
   long long b = (total + block - 1) / block;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   return static_cast<int>(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
@@ -421,7 +421,7 @@ extern "C" int mega_copy_rows_batch(const mega_copy_job* jobs_host, int n_jobs, 
     if (words / 4 > most) most = words / 4;
   }
   for (int i = n_jobs; i < kMaxCopyJobs; ++i) jobs.j[i] = jobs_host[0];
-  dim3 grid(grid_for(most, 256) > 148 ? 148 : grid_for(most, 256), n_jobs);
+  dim3 grid(grid_for(most, 256) > 132 ? 132 : grid_for(most, 256), n_jobs);
   copy_rows_batch_kernel<<<grid, 256, 0, stream>>>(jobs);
   MEGA_CUDA_CHECK(cudaGetLastError());
   return MEGA_OK;

@@ -219,7 +219,7 @@ __global__ void dff_warp_scale_kernel(const T* __restrict__ key, int ld, int cha
 
 static int grid_for(long long total, int block) {
   long long b = (total + block - 1) / block;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   return static_cast<int>(b < 1 ? 1 : (b > cap ? cap : b));
 }
 

@@ -45,7 +45,7 @@ extern "C" int mega_image_transform_u8(const unsigned char* src, int src_h, int 
   g.to_bgr255 = to_bgr255 ? 1 : 0;
   const long long total = static_cast<long long>(out_h) * out_w;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;
+  if (blocks > 132LL * 16) blocks = 132LL * 16;
   mega::image_transform_kernel<<<static_cast<int>(blocks), 256, 0, stream>>>(total, g, src, out);
   MEGA_CUDA_CHECK(cudaGetLastError());
   return MEGA_OK;

@@ -7,7 +7,7 @@
 // Here nothing of that is materialised: for every (query n, key m) pair the four log-ratios,
 // the 64 sin/cos features, the 64->16 projection, ReLU, log and the scaled logit are computed in
 // registers and the soft-max is taken in place over the [G,N,M] logits produced by the
-// tcgen05 Q.K^T GEMM. One CTA per query row; two passes over its [16,M] slice (L2-resident):
+// wgmma Q.K^T GEMM. One CTA per query row; two passes over its [16,M] slice (L2-resident):
 // logits + online (max, sum), then normalise.
 #include <stdlib.h>
 #include <cuda_fp16.h>

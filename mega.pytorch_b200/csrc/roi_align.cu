@@ -627,7 +627,7 @@ extern "C" int mega_roi_align_forward_nchw(const float* input, int batch, int ch
   const long long total = static_cast<long long>(num_rois) * channels * pooled_h * pooled_w;
   if (total == 0) return MEGA_OK;  // ROIAlign_cuda.cu:278-281
   long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
   roi_align_nchw_kernel<<<static_cast<int>(blocks), 256, 0, stream>>>(input, channels, height, width, rois, total,
                                                                       spatial_scale, pooled_h, pooled_w,
                                                                       sampling_ratio, output);

@@ -6,7 +6,7 @@
 //   mega_channel_sum_nchw                 <- the grad_bias `ones` GEMM      (deform_conv_cuda.cu:667-672)
 //   mega_deform_psroi_pooling_backward    <- _C.deform_psroi_pooling_backward (csrc/deform_pool.h:41-69)
 // The per-item bodies live in train_ops.cuh (shared with the host build that the CPU tests check against the oracle);
-// the kernels below are grid-stride loops over items, sized to a multiple of the 148 SMs. All of them are HBM / L2
+// the kernels below are grid-stride loops over items, sized to a multiple of the 132 SMs. All of them are HBM / L2
 // atomic bound: items are numbered so that a warp touches consecutive addresses of one plane.
 #include "common.cuh"
 #include "mega_b200.h"
@@ -90,7 +90,7 @@ __global__ void deform_psroi_bwd_kernel(long long total, PsRoiGeom g, const floa
 
 static int grid_for(long long total, int block) {
   long long b = (total + block - 1) / block;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   return static_cast<int>(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
@@ -197,7 +197,7 @@ extern "C" int mega_channel_sum_nchw(const float* x, int batch, int channels, in
   if (batch <= 0 || channels <= 0 || plane <= 0) return MEGA_OK;
   const int warps = 8;
   int blocks = (channels + warps - 1) / warps;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   channel_sum_nchw_kernel<<<blocks, warps * 32, 0, stream>>>(x, batch, channels, plane, out);
   MEGA_CUDA_CHECK(cudaGetLastError());
   return MEGA_OK;

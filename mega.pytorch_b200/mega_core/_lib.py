@@ -86,8 +86,6 @@ lib.mega_nms_host.restype = c_int
 lib.mega_roi_align_forward_nchw_host.argtypes = [ctypes.c_void_p, c_int, c_int, c_int, c_int, ctypes.c_void_p, c_int,
                                                  ctypes.c_float, c_int, c_int, c_int, c_int, ctypes.c_void_p]
 lib.mega_roi_align_forward_nchw_host.restype = c_int
-lib.mega_set_split16_a_tmem.argtypes = [c_int]
-lib.mega_set_split16_a_tmem.restype = c_int
 lib.mega_set_split3_seg_len.argtypes = [c_int]
 lib.mega_set_split3_seg_len.restype = c_int
 lib.mega_set_tf32_rounding.argtypes = [c_int]
@@ -230,7 +228,7 @@ lib.mega_vid_match_host.restype = _i
 EXPORTS = [
     "mega_last_error", "mega_abi_version", "mega_device_ok", "mega_conv_gemm", "mega_conv_gemm_tf32", "mega_conv_gemm_workspace_bytes", "mega_set_tf32_rounding",
     "mega_conv_chain_plan_bytes", "mega_conv_chain_encode", "mega_conv_chain_launch", "mega_conv_chain_set_trace",
-    "mega_conv_chain_encode2", "mega_conv_chain_launch2", "mega_set_split3_seg_len", "mega_set_split16_a_tmem", "mega_conv_chain_set_trace2", "mega_nms_host", "mega_roi_align_forward_nchw_host",
+    "mega_conv_chain_encode2", "mega_conv_chain_launch2", "mega_set_split3_seg_len", "mega_conv_chain_set_trace2", "mega_nms_host", "mega_roi_align_forward_nchw_host",
     "mega_nms_workspace_bytes", "mega_nms", "mega_rpn_select_workspace_bytes", "mega_rpn_select",
     "mega_roi_align_forward_nchw", "mega_roi_align_forward_nhwc", "mega_stem_im2col", "mega_maxpool3x3s2_nhwc",
     "mega_gather_rows", "mega_copy_rows", "mega_copy_rows_batch", "mega_transpose_2d", "mega_relation_softmax", "mega_box_postprocess_workspace_bytes",

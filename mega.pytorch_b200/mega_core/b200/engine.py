@@ -1,7 +1,7 @@
-"""Per-frame inference engine for the MEGA / single-frame paths on B200.
+"""Per-frame inference engine for the MEGA / single-frame paths on H100.
 
 Host-side orchestration only: every tensor operation below is a launch of a hand-written
-sm_100a kernel through the C ABI (`ops.*`); torch supplies device memory and the stream.
+sm_90a kernel through the C ABI (`ops.*`); torch supplies device memory and the stream.
 
 Restructuring relative to the reference (all exact re-associations or de-duplications of the
 same arithmetic, see DESIGN.md):
@@ -609,7 +609,7 @@ class WindowedEngine(HeadCommon):
             finally:
                 ops.WS_LANE[0] = 0
         side_ctas = max(4, n)       # the proposal selection runs one latency-bound CTA per image beside the res5 chain
-        mc = 148 - side_ctas
+        mc = 132 - side_ctas
         dual = self.chained and ops.DUAL_CHAIN[0] and n >= ops.DUAL_MIN_IMAGES and n % 2 == 0
         with ops.chain(self._chains, ("res5", tuple(feats.shape), dual), self.dev, enabled=self.chained, max_ctas=mc,
                        interleave=dual) as ch:
@@ -1095,13 +1095,12 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
         return dets
 
     # ---- two launch sequences side by side: the aggregation of a batch of key frames uses the GPU badly on its own (GEMMs of
-    #      300-675 rows = 24-48 tiles on 148 SMs, latency-bound soft-max and NMS kernels: ~25 % of the step at ~1/3 occupancy),
+    #      300-675 rows = 24-48 tiles on 132 SMs, latency-bound soft-max and NMS kernels),
     #      and the per-frame branch of the NEXT batch does not depend on it. stepn_pipelined issues the two on two streams: the
     #      block scheduler fills the SMs a draining branch kernel frees with aggregation CTAs and vice versa. PIPE_SMS
     #      (MEGA_B200_PIPE_SMS="branch,aggregation") optionally caps the persistent grids so that the two sequences own
-    #      disjoint SMs (ops.sm_limit) -- measured on a B200, strict mode, 4 key frames per step (sequential: 18.5 ms):
-    #      no caps 17.65 ms; aggregation capped at 32: 20.7; 132 + 16: 23.7; 140 + 8: 35.1 (a capped aggregation becomes the
-    #      critical path: its kernels are latency-bound, fewer SMs make each of them slower). Default: no caps.
+    #      disjoint SMs (ops.sm_limit); a capped aggregation tends to become the critical path (its kernels are
+    #      latency-bound, fewer SMs make each of them slower). Default: no caps.
     PIPE_SMS = tuple(int(v) for v in os.environ.get("MEGA_B200_PIPE_SMS", "0,0").split(","))
 
     @_with_precision
@@ -1113,8 +1112,8 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
         # chain kernels (fp16 mode) hold grid-wide barriers: two of them may only run side by side on DISJOINT SM budgets (a
         # CTA that spins for peers which cannot become resident would deadlock), so that mode always runs capped
         caps = self.PIPE_SMS
-        if self.chained and not (caps[0] > 0 and caps[1] > 0 and caps[0] + caps[1] + 8 <= 148):
-            caps = (124, 16)
+        if self.chained and not (caps[0] > 0 and caps[1] > 0 and caps[0] + caps[1] + 8 <= 132):
+            caps = (108, 16)
         main = torch.cuda.current_stream(self.dev)
         if getattr(self, "_pipe_stream", None) is None:
             self._pipe_stream = torch.cuda.Stream(device=self.dev)
@@ -1474,7 +1473,7 @@ class BaseEngine(HeadCommon, MlpHeadMixin):
 class FlowNetS:
     """FlowNetS.forward, method "fgfa" (modeling/backbone/flownet.py:54-118) over NHWC activations.
 
-    Every layer is a launch of the tcgen05 implicit-GEMM kernel:
+    Every layer is a launch of the wgmma implicit-GEMM kernel:
       * flow_conv1 (7x7 / stride 2 over 6 channels): the image pairs are stored with 8 channels per pixel, so the 7 taps of
         one filter row are 56 (+8 zero-weighted) CONTIGUOUS elements -- one K slab per filter row through an overlapping
         strided view (pixel pitch 16 elements = 2 input pixels), 7 k-blocks instead of a 49-tap / 6-channel gather;

@@ -14,7 +14,7 @@ LAUNCHES = [0]
 
 
 def _launch_conv_gemm(d):
-    """single choke point of the tcgen05 kernel (bench.py wraps it with CUDA events for the roofline)"""
+    """single choke point of the wgmma kernel (bench.py wraps it with CUDA events for the roofline)"""
     if _CHAIN_MODE[0] == "record":
         _CHAIN_REC[0].append(_copy_desc(d))
         return
@@ -162,9 +162,8 @@ class chain(object):
 
 # interleaved (depth-2) chains for the per-frame branch when the image batch splits into two halves
 import os as _os
-# Measured on a B200 (backbone chain, fp16, 600x1000; ms for 2 / 4 / 8 images): one chain 1.61 / 2.49 / 4.06, two
-# interleaved lanes 1.87 / 2.33 / 3.75 -- lanes of a single image leave too few tiles per layer, so the engine interleaves
-# from 4 images on (DUAL_MIN_IMAGES); MEGA_B200_DUAL_CHAIN=0 switches it off
+# Lanes of a single image leave too few tiles per layer, so the engine interleaves from 4 images on (DUAL_MIN_IMAGES);
+# MEGA_B200_DUAL_CHAIN=0 switches it off
 DUAL_CHAIN = [_os.environ.get("MEGA_B200_DUAL_CHAIN", "1") != "0"]
 DUAL_MIN_IMAGES = 4
 
@@ -480,7 +479,7 @@ def _autotune_chain(d):
 def pick_config(cout, m_tiles, batch, kb_per_tile, out_f16=False):
     """(block_n, stream_k) when no autotuned entry exists. Deep reductions balance best at k-block
     granularity (stream-K, widest tile); shallow ones run whole tiles, with the tile width chosen to
-    minimise waves x bytes staged per k-block on 148 SMs."""
+    minimise waves x bytes staged per k-block on 132 SMs."""
     if kb_per_tile >= 48:
         for bn in (32, 64, 128):
             if cout <= bn and not (out_f16 and bn % 64):
@@ -495,7 +494,7 @@ def pick_config(cout, m_tiles, batch, kb_per_tile, out_f16=False):
         if bn >= 2 * cout and bn > (64 if out_f16 else 32):
             continue
         tiles = m_tiles * (-(-cout // bn)) * batch
-        cost = (-(-tiles // 148)) * (128 + bn)
+        cost = (-(-tiles // 132)) * (128 + bn)
         if best is None or cost < best[0] or (cost == best[0] and bn > best[1]):
             best = (cost, bn)
     return best[1], 0
@@ -509,7 +508,7 @@ def conv_gemm(a, w, out, *, taps=(1, 1), dil=1, pad=0, scale=None, bias=None, re
               relu=False, tile=None, block_n=None, cout=None, k=None, batch=1, a_c_off=0,
               a_n_off=0, b_k_off=0, b_n_off=0, out_c_off=0, out_n_off=0, res_c_off=0, res_n_off=0, bias_z_off=0,
               max_ctas=0, stream_k=None, out_hw=None, n_img=None, stride=(1, 1), pad_w=None):
-    """out[n,h,w,:] = act(scale * conv(a, w) + bias + residual)   (tcgen05 tensor cores, fp32 accumulate)
+    """out[n,h,w,:] = act(scale * conv(a, w) + bias + residual)   (wgmma tensor cores, fp32 accumulate)
 
     a   : [N,H,W,C] fp32 or fp16 view (innermost stride 1; other strides multiples of 16 bytes)
     w   : [taps, rows, K] same dtype as a (K contiguous)

@@ -6,7 +6,7 @@ increments of the group's earlier frames, after its last read the rest (the refe
 replaces the replicated "state" part of dist_step (~0.7 ms per foreign frame) by three latency-bound collectives. The
 launches of the rank's own frame are those of MegaEngine._aggregate_split(owner), so detections are bit-identical to
 dist_step for any world size. Schedule tables, the NCCL / in-process drivers and the self-check live in parallel.py; the
-evidence (symbolic proof, engine code on CPU stand-ins, gloo, bit-identity on a B200) is listed in DESIGN.md section 6."""
+evidence (symbolic proof, engine code on CPU stand-ins, gloo, bit-identity on one GPU) is listed in DESIGN.md section 6."""
 import torch
 
 from . import ops

@@ -1,6 +1,6 @@
 """Differentiable wrappers of the `_C` ops with the reference's layer names (layers/roi_align.py, roi_pool.py,
 sigmoid_focal_loss.py, smooth_l1_loss.py, dcn/deform_conv_func.py, dcn/deform_conv_module.py, dcn/deform_pool_func.py,
-dcn/deform_pool_module.py). Forward and backward both run on the sm_100a kernels of libmega_b200.so through
+dcn/deform_pool_module.py). Forward and backward both run on the sm_90a kernels of libmega_b200.so through
 `mega_core._C`; nothing here has a CPU path. None of these layers is reached by the VID inference configs -- they
 complete the operator API behind which `tools/train_net.py`-style callers find the same names (SURVEY.md 8b, 8f row 3).
 

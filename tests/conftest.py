@@ -11,7 +11,7 @@ for p in (ROOT, PKG):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (H100); run with -m gpu")
 
 
 @pytest.fixture(scope="session")
@@ -20,5 +20,5 @@ def cuda_dev():
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     from mega_core import _lib
-    assert _lib.lib.mega_device_ok() == 1, "libmega_b200 kernels are built for sm_100a (B200) only"
+    assert _lib.lib.mega_device_ok() == 1, "libmega_b200 kernels are built for sm_90a (H100) only"
     return torch.device("cuda:0")

@@ -1,7 +1,7 @@
 """Test harness: an fp32 'shadow' of ops.conv_gemm built from torch ops (cuBLAS/cuDNN with TF32 off).
 
 Used only by tests/tools to separate LOGIC errors of the engine orchestration from TF32 rounding
-of the tcgen05 kernel: with the shadow installed every dense contraction is exact fp32 while all
+of the wgmma kernel: with the shadow installed every dense contraction is exact fp32 while all
 other kernels (NMS, RPN selection, ROIAlign, relation soft-max, post-processing) stay ours."""
 import contextlib
 

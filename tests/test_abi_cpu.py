@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(_lib.lib, s), "libmega_b200.so does not export %s" % s
     assert sorted(_lib.EXPORTS) == syms
-    assert _lib.lib.mega_abi_version() == 6
+    assert _lib.lib.mega_abi_version() == 7
 
 
 def test_no_cpu_fallback():

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM kernel against torch fp32 (CPU) references.
+"""GPU parity of the wgmma implicit-GEMM kernel against torch fp32 (CPU) references.
 
 TF32 operands (10-bit mantissa, round-to-nearest on load) with fp32 accumulation: the stated
 tolerance is max|err| <= 4e-3 x RMS(output) (observed 1.5e-3..2.1e-3, identical to cuBLAS TF32).

@@ -147,7 +147,7 @@ def test_mega_r101_tf32_matches_reference_fixture(cuda_dev):
 
 def test_mega_r101_fp32x3_product_path_matches_reference_fixture(cuda_dev):
     """The PRODUCT path in its strict-parity arithmetic (EngineConfig(precision="fp32x3"): every dense contraction on
-    the tcgen05 tensor cores as a 3xTF32 split with the accumulator re-started every 4 k-blocks, ~2e-6 relative error)
+    the wgmma tensor cores as a 3xTF32 split with the accumulator re-started every 4 k-blocks, ~2e-6 relative error)
     against the reference's outputs: every proposal and every detection reproduced; class logits within 1e-2
     (measured 1.2e-3 .. 5.9e-3, logit RMS 0.76). The 1e-3 bar of the north star is met by the exact-fp32 shadow test
     above (<= 7e-4, i.e. two fp32 evaluations that merely SUM in a different order already differ by ~1e-3 on this

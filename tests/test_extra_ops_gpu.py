@@ -84,7 +84,7 @@ def test_callable_submodules_match_the_oracle_pieces(cuda_dev):
     parts (generalized_rcnn_mega.py:145-158, :173-175, :208; rpn/rpn.py:213-243; extractors :657-676, :885-896) -- served
     by the detector's engine, against the oracle's functions of the same steps on the same inputs."""
     import mega_oracle as mo
-    from mega_core.b200 import synth
+    from mega_core.b200 import ops, synth
     from mega_core.modeling.detector import build_detection_model_from_state_dict
     from mega_core.structures.image_list import to_image_list
     sd = synth.make_state_dict("mega_r101_tiny", seed=3)
@@ -126,6 +126,10 @@ def test_callable_submodules_match_the_oracle_pieces(cuda_dev):
     fe.update_global(x)
     eng = model.engine
     assert eng.glob_pushed == 1 and eng.mem_pushed == 0
-    assert torch.allclose(eng.glob_x[:75].float(), x, atol=1e-6)
+    got = eng.glob_x[:75]
+    if ops.is_split16(eng.glob_x):     # the strict engine stores its rows split (hi + lo fp16): decode them
+        got = ops.unpack_split16(got.contiguous(), torch.empty_like(got, dtype=torch.float32))
+    assert not ops.is_split16(x)       # update_global packs a copy: the caller's rows stay plain fp32
+    assert torch.allclose(got.float(), x, atol=1e-6)
     with pytest.raises(NotImplementedError):
         fe((dfeats,), [key[0]], pre_calculate=False)

@@ -65,7 +65,7 @@ def test_fixture_covers_the_baseline_configuration():
 
 
 def test_mega_600x1000_strict_mode_meets_the_logit_bar(cuda_dev, gold_and_frames):
-    """fp32x3 (every contraction on the tcgen05 tensor cores as a 3xTF32 split): every proposal and every detection of the
+    """fp32x3 (every contraction on the wgmma tensor cores as a 3xTF32 split): every proposal and every detection of the
     reference reproduced on every check frame (memory empty, filling and full), class logits within the north star's 1e-3
     at the 99th percentile and within 2e-2 at the maximum (the reference's own fp32-vs-fp64 distances: 7.7e-5 / 1.05e-2)"""
     rows = _run(cuda_dev, gold_and_frames, "fp32x3")

@@ -96,28 +96,6 @@ def test_conv_3xfp16_matches_fp64(cuda_dev, case):
     assert err < TOL, err
 
 
-@pytest.mark.parametrize("case", [
-    (1, 38, 63, 256, 256, 3, 1, True, None, True, 128, 0, 1.0),
-    (1, 38, 63, 256, 1024, 1, 1, True, "split", True, 128, 0, 1.0),
-    (2, 38, 63, 1024, 256, 1, 1, True, None, True, 128, 1, 1.0),
-    (1, 19, 21, 96, 80, 3, 1, False, None, False, 64, 0, 1.0),
-])
-def test_a_operand_through_tensor_memory_is_bit_identical(cuda_dev, case):
-    """mega_set_split16_a_tmem(1): every staged A tile is copied to tensor memory (tcgen05.cp) and the MMAs run in the TS form --
-    the same products in the same order, so the outputs must not change by a bit"""
-    from mega_core._lib import lib
-    n, h, w, cin, cout, ks, dil, relu, res, osplit, bn, sk, ws = case
-    outs = []
-    for mode in (0, 1):
-        old = lib.mega_set_split16_a_tmem(mode)
-        try:
-            outs.append(_conv_case(cuda_dev, n, h, w, cin, cout, ks, dil, relu, res, osplit, seed=7, block_n=bn, stream_k=sk,
-                                   wscale=ws, want_output=True))
-        finally:
-            lib.mega_set_split16_a_tmem(old)
-    assert outs[0][0] < TOL and torch.equal(outs[0][1], outs[1][1])
-
-
 def test_deep_reduction_as_taps_matches_fp64(cuda_dev):
     """the l_fcs[0] form: [rows, K] x [K/64 taps][1024][64] with K = 64 x 392, stream-K over a 12544-deep reduction"""
     from mega_core.b200 import ops

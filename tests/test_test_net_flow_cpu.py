@@ -29,8 +29,23 @@ def test_imports_of_tools_test_net_resolve():
     assert setup_logger("mega_core.test", "", 1) is not None
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/configs"), reason="reference checkout not present")
+def _reference_configs(root):
+    """the reference's YAML configs, written back from their stored contents (tests/golden/reference_configs.json, the
+    key/value data of configs/*.yaml of the original project) to <root>/configs/..."""
+    import json
+    import yaml
+    with open(os.path.join(ROOT, "tests", "golden", "reference_configs.json")) as fh:
+        configs = json.load(fh)
+    for name, data in configs.items():
+        path = os.path.join(root, name)
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        with open(path, "w") as fh:
+            yaml.safe_dump(data, fh)
+    return root
+
+
 def test_reference_yaml_configs_merge_and_drive_the_loader(tmp_path):
+    ref = _reference_configs(str(tmp_path / "ref"))
     from mega_core.config import cfg as base
     from mega_core.config.paths_catalog import DatasetCatalog
     from mega_core.data import make_data_loader
@@ -42,22 +57,22 @@ def test_reference_yaml_configs_merge_and_drive_the_loader(tmp_path):
                                ("dff", "configs/DFF/vid_R_101_C4_DFF_1x.yaml", "GeneralizedRCNNDFF"),
                                ("base", "configs/vid_R_50_C4_1x.yaml", "GeneralizedRCNN")):
         cfg = base.clone()
-        cfg.merge_from_file("/root/reference/configs/BASE_RCNN_1gpu.yaml")          # test_net.py:75-78
-        cfg.merge_from_file(os.path.join("/root/reference", yaml))
+        cfg.merge_from_file(os.path.join(ref, "configs/BASE_RCNN_1gpu.yaml"))          # test_net.py:75-78
+        cfg.merge_from_file(os.path.join(ref, yaml))
         cfg.merge_from_list(["MODEL.DEVICE", "cpu", "DATALOADER.NUM_WORKERS", 0])
         cfg.freeze()
         assert cfg.MODEL.VID.METHOD == method and cfg.MODEL.META_ARCHITECTURE == arch and cfg.TEST.IMS_PER_BATCH == 1
         model = build_detection_model(cfg)
         assert type(model).__name__ == arch
     # the MEGA config drives the loader over a tree laid out like datasets/ILSVRC2015
-    make_tree(str(tmp_path))
+    make_tree(str(tmp_path / "data"))
 
     class Catalog(DatasetCatalog):
-        DATA_DIR = str(tmp_path)
+        DATA_DIR = str(tmp_path / "data")
 
     cfg = base.clone()
-    cfg.merge_from_file("/root/reference/configs/BASE_RCNN_1gpu.yaml")
-    cfg.merge_from_file("/root/reference/configs/MEGA/vid_R_101_C4_MEGA_1x.yaml")
+    cfg.merge_from_file(os.path.join(ref, "configs/BASE_RCNN_1gpu.yaml"))
+    cfg.merge_from_file(os.path.join(ref, "configs/MEGA/vid_R_101_C4_MEGA_1x.yaml"))
     cfg.merge_from_list(["DATALOADER.NUM_WORKERS", 0])
     assert tuple(cfg.DATASETS.TEST) == ("VID_val_videos",)
     np.random.seed(0)

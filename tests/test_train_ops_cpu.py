@@ -7,7 +7,7 @@ deform_psroi_pooling_backward; SURVEY.md section 8b / 8f row 3):
   2. the per-item device functions of csrc/train_ops.cuh, compiled for the host (tests/native/train_ops_host.cpp, same
      entry-point names and prototypes as the C ABI) and run item by item, reproduce those oracles when driven by the
      product's own host code: the tests patch the host build over the ctypes handles of libmega_b200.so (and a torch
-     matmul over the tcgen05 GEMM wrapper) and call `mega_core._C.*` on CPU tensors. The index arithmetic and gradient
+     matmul over the wgmma GEMM wrapper) and call `mega_core._C.*` on CPU tensors. The index arithmetic and gradient
      formulas of the CUDA kernels, the argument order of every ctypes call and the operand re-layouts of _C.py are thus
      verified here; tests/test_zz_train_ops_gpu.py repeats the comparison on the GPU, where only the launch
      configuration and the GEMM calls are new. (The patching exists in this test only: the product has no CPU path.)

@@ -5,7 +5,7 @@ tests/test_train_ops_cpu.py). Scatter kernels accumulate with red.global.add.f32
 reference's atomicAdd does, so float results are compared to 1e-5-level tolerances; arg-max indices are exact.
 Order inside the file (the GPU tier runs with -x): most certain first -- integer-exact image transform, the simple
 scatter kernels, the engine-level wavefront / DFF checks (all-existing kernels in a new order), then the ops that also
-drive the tcgen05 GEMM with shapes it has not seen (deformable-conv backward, the layer wrappers).
+drive the wgmma GEMM with shapes it has not seen (deformable-conv backward, the layer wrappers).
 (This file sorts last on purpose: these kernels were added after the last full GPU session of round 1 and verified on
 the CPU first, through their host builds; a surprise here must not hide the hot-path tests. First B200 run: 20 of 21
 passed unchanged, see profiles/r01_summary.md.)"""
@@ -284,7 +284,7 @@ def test_deform_conv_backward(cuda_dev, modulated, groups, dg, stride, pad, dil)
 
 
 def test_layers_autograd_on_device(cuda_dev):
-    """mega_core.layers wrappers: forward and backward both on the sm_100a kernels"""
+    """mega_core.layers wrappers: forward and backward both on the sm_90a kernels"""
     import train_ops_oracle as to
     from mega_core import layers
     from mega_core.b200 import ops
@@ -348,7 +348,7 @@ def test_nvjpeg_decode_feeds_the_transform(cuda_dev):
 def test_two_key_frames_per_call_on_device(cuda_dev):
     """MegaEngine.step2_batched (per-frame branch of two key frames as one batch of four images; bit-identical to two
     step_batched calls on the CPU stand-ins) on the device: a different batch size moves the stream-K split points of the
-    tcgen05 GEMMs, so the comparison with two single-frame steps is statistical (the fp16 re-association noise bound of
+    wgmma GEMMs, so the comparison with two single-frame steps is statistical (the fp16 re-association noise bound of
     the frame-parallel test); the window / global rings, which are plain copies of identical payload rows up to that
     noise, must stay close as well."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))

@@ -74,7 +74,7 @@ import fp32_shadow as _fs  # noqa: E402
 
 
 def per_gemm_audit():
-    """strict mode: run every conv_gemm of two frames twice -- tcgen05 3xTF32 and the fp64 shadow on the SAME
+    """strict mode: run every conv_gemm of two frames twice -- wgmma 3xTF32 and the fp64 shadow on the SAME
     inputs -- and report the worst relative error with the call's signature"""
     worst = []
     real = ops.conv_gemm

@@ -1,4 +1,4 @@
-"""Three representative contractions of the strict mode (3xTF32 with the A operand in TMEM; --split16: 3xFP16 on split-fp16 tensors) at the sizes of a 4-key-frame step
+"""Three representative contractions of the strict mode (3xTF32; --split16: 3xFP16 on split-fp16 tensors) at the sizes of a 4-key-frame step
 (8 images of 600x1000), timed with CUDA events and -- under `ncu --profile-from-start off` -- profiled one launch each:
 res4 3x3 (K = 2304 -> 256), RPN head 3x3 (K = 9216 -> 1024), res4 1x1 expand (K = 256 -> 1024, residual).
     ncu --set full --clock-control none --import-source on --profile-from-start off -o gpurun_out/strict python tools/strict_gemm_probe.py"""
@@ -16,7 +16,6 @@ from mega_core.b200 import ops  # noqa: E402
 dev = torch.device("cuda:0")
 g = torch.Generator().manual_seed(0)
 n, h, w = 8, 38, 63
-ops.load_tuned(os.path.join(ROOT, "mega.pytorch_b200", "mega_core", "b200", "tuned_b200.json"))
 ops.AUTOTUNE[0] = True
 
 
@@ -47,11 +46,7 @@ if "--split16" in sys.argv and "--more" in sys.argv:
     cases += [("rpn head 1x1 1024->75, block_n 64", lambda: ops.conv_gemm(x1024, whead, ohead, bias=bi[:75], cout=75, block_n=64), 2 * n * h * w * 75 * 1024),
               ("rpn head 1x1 1024->75, block_n 128", lambda: ops.conv_gemm(x1024, whead, ohead, bias=bi[:75], cout=75, block_n=128), 2 * n * h * w * 75 * 1024),
               ("res5 3x3 dil 2 512->512", lambda: ops.conv_gemm(x512, w5, o512, taps=(3, 3), dil=2, pad=2, bias=bi[:512], relu=True), 2 * n * h * w * 512 * 4608),
-              ("res5 3x3 dil 2 512->512, 140 CTAs", lambda: ops.conv_gemm(x512, w5, o512, taps=(3, 3), dil=2, pad=2, bias=bi[:512], relu=True, max_ctas=140), 2 * n * h * w * 512 * 4608)]
-if "--a-tmem" in sys.argv:
-    from mega_core._lib import lib
-    lib.mega_set_split16_a_tmem(1)
-    print("A operand through tensor memory (tcgen05.cp + TS-form MMAs)")
+              ("res5 3x3 dil 2 512->512, 124 CTAs", lambda: ops.conv_gemm(x512, w5, o512, taps=(3, 3), dil=2, pad=2, bias=bi[:512], relu=True, max_ctas=124), 2 * n * h * w * 512 * 4608)]
 with ops.precision("fp32x3"):
     for name, fn, flops in cases:
         for _ in range(3):
