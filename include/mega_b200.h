@@ -112,7 +112,12 @@ typedef struct mega_conv_gemm_desc {
    * normal fp16 numbers (mega_core.b200.ops.pack_weights_split16). */
   int res_split;
   float acc_scale;
-  int reserved_v6;
+  /* (zero = previous behaviour) group_width in {8, 16, 32, 64}: the launch is a grouped convolution with groups of that
+   * many channels in the 64-channel batched layout -- batch = channels / 64, block_n = cout = k_per_tap = b_k = 64,
+   * a_c_off = b_n_off = out_c_off = res_c_off = 64, b_k_off = 0, b weights [taps][channels][64] block-diagonal (row co holds
+   * the weights of input channels 64 (co / 64) + j, zero outside the gw x gw diagonal blocks; mega_core.b200.ops
+   * .pack_grouped_conv). The MMAs then cover the diagonal blocks only; the result equals the same launch with 0. */
+  int group_width;
 } mega_conv_gemm_desc;
 
 /* fp32 <-> split-fp16 (format above) over n_values contiguous values (multiple of 32, 128-byte aligned); pack may run in

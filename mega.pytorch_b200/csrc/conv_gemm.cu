@@ -142,6 +142,17 @@ int encode_conv_gemm_problem(const mega_conv_gemm_desc* d, CUtensorMap* tmA_p, C
   } else {
     MEGA_ARG_CHECK(d->res_split == 0, "conv_gemm: res_split needs precision 3");
   }
+  if (d->group_width != 0) {
+    const int gw = d->group_width;
+    MEGA_ARG_CHECK(gw == 8 || gw == 16 || gw == 32 || gw == 64, "conv_gemm: group_width must be 8, 16, 32 or 64 (got %d)", gw);
+    MEGA_ARG_CHECK(d->block_n == 64 && d->cout == 64 && d->k_per_tap == 64 && d->b_k == 64 && d->a_c_off == 64 &&
+                       d->b_n_off == 64 && d->out_c_off == 64 && d->b_k_off == 0 && (d->residual == nullptr || d->res_c_off == 64),
+                   "conv_gemm: group_width needs the 64-channel batched layout (block_n = cout = k_per_tap = b_k = 64, "
+                   "a_c_off = b_n_off = out_c_off = res_c_off = 64, b_k_off = 0; got block_n %d cout %d k %d b_k %d offsets "
+                   "%d %d %d %d %d)", d->block_n, d->cout, d->k_per_tap, d->b_k, d->a_c_off, d->b_n_off, d->out_c_off,
+                   d->res_c_off, d->b_k_off);
+    MEGA_ARG_CHECK(d->b_lo_tap_off == 0, "conv_gemm: group_width does not take pre-split weights (b_lo_tap_off)");
+  }
   const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                                      : (g_tf32_round && !strict && !pk) ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32
                                                                  : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
@@ -321,6 +332,16 @@ extern "C" int mega_conv_gemm(const mega_conv_gemm_desc* d, void* stream_v) {
   const bool out16 = d->out_f16 != 0;
   dim3 grid(static_cast<unsigned>(ctas), 1, 1);
   const int pdl = d->pdl ? 1 : 0;
+  // grouped launches (block_n 64, checked by the encoder) issue only the diagonal blocks; with one group per 64 channels
+  // (gw 64) that is the dense k-block. The layer chain runs grouped layers with the dense issue (same result).
+  const int gw = d->group_width == 64 ? 0 : d->group_width;
+  if (gw != 0) {
+    if (d->precision == kModeF16x3)
+      return launch_conv_gemm_f16x3_grouped(gw, out16 ? 1 : 0, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    if (f16) return launch_conv_gemm_f16_grouped(gw, out16 ? 1 : 0, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    if (strict) return launch_grouped<4, kModeSplit3, false>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    return launch_grouped<5, kModeTf32, false>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+  }
   if (d->precision == kModeF16x3)
     return launch_conv_gemm_f16x3(d->block_n, out16 ? 1 : 0, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
   if (f16) return launch_conv_gemm_f16(d->block_n, out16 ? 1 : 0, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);

@@ -30,4 +30,10 @@ int launch_conv_gemm_f16(int block_n, int out_f16, const CUtensorMap& tmA, const
   return MEGA_ERR_ARG;
 }
 
+int launch_conv_gemm_f16_grouped(int gw, int out_f16, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
+                                 const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid, cudaStream_t stream, int pdl) {
+  return out_f16 ? launch_grouped<5, kModeF16, true>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
+                 : launch_grouped<5, kModeF16, false>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+}
+
 }  // namespace mega

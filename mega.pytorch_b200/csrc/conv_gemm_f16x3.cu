@@ -20,4 +20,10 @@ int launch_conv_gemm_f16x3(int block_n, int out_split, const CUtensorMap& tmA, c
   return MEGA_ERR_ARG;
 }
 
+int launch_conv_gemm_f16x3_grouped(int gw, int out_split, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
+                                   const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid, cudaStream_t stream, int pdl) {
+  return out_split ? launch_grouped<5, kModeF16x3, true>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
+                   : launch_grouped<5, kModeF16x3, false>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+}
+
 }  // namespace mega

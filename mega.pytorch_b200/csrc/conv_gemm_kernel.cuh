@@ -271,6 +271,88 @@ __device__ __forceinline__ void mma_kblock(float (&d)[BN / 2], uint32_t a_addr, 
   wgmma_commit();
 }
 
+// One k-block of a grouped convolution (mega_conv_gemm_desc::group_width = GW in {8, 16, 32}; block_n 64 and 64 channels per
+// batch entry, so the staged weight tile is block-diagonal): k-step K, whose KS channels ch0 .. ch0 + KS feed only the
+// output columns of their own groups, issues one wgmma of width N = max(GW, KS) over those columns -- B rows [col0, col0 + N)
+// (8-row swizzle atoms: +8 col0 in descriptor units) into accumulator registers [col0 / 2, col0 / 2 + N / 2) (the m64nNk*
+// fragment keeps every 8-column block in 4 consecutive registers). The products it leaves out are exact zeros, so the
+// accumulator equals the dense k-block's. A k-block touches only some columns: mma_pass clears the accumulator at the start
+// of a segment and every MMA accumulates. KC: which 32-channel half of the tap the k-block holds (32-value K slabs).
+// Grouped launches run their own kernel instantiations (GW template argument): a runtime choice between this issue and
+// the dense one inside a kernel would make ptxas serialise all of its wgmma groups.
+template <int V>
+struct IntC {
+  static constexpr int value = V;
+};
+template <int K, int KN, class F>
+__device__ __forceinline__ void static_for(F&& f) {
+  if constexpr (K < KN) {
+    f(IntC<K>());
+    static_for<K + 1, KN>(f);
+  }
+}
+
+template <int MODE, int GW, int KC>
+__device__ __forceinline__ void mma_kblock_grouped(float (&d)[32], uint32_t a_addr, uint32_t b_addr, uint32_t b_lo_addr,
+                                                   const int wtid) {
+  constexpr int KS = (MODE == kModeF16 || MODE == kModeF16x3) ? 16 : 8;    // channels per k-step
+  constexpr int N = GW > KS ? GW : KS;
+  constexpr int NK = MODE == kModeF16x3 ? 2 : 4;                           // k-steps per k-block
+  const uint64_t adesc = wgmma_desc_sw128(a_addr);
+  const uint64_t bdesc = wgmma_desc_sw128(b_addr);
+  if constexpr (MODE == kModeSplit3) {
+    const int g = (wtid >> 5) * 16 + ((wtid & 31) >> 2), t = wtid & 3;
+    const uint64_t blo = wgmma_desc_sw128(b_lo_addr);
+    uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int r = g + (e & 1) * 8, col = 8 * k + t + (e >> 1) * 4;
+        float x;
+        asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(a_addr + r * 128 + ((((col >> 2) ^ (r & 7)) << 4) | ((col & 3) << 2))));
+        const uint32_t h = __float_as_uint(x) & 0xffffe000u;
+        ahi[k][e] = h;
+        alo[k][e] = __float_as_uint(x - __uint_as_float(h));
+      }
+    }
+    wgmma_fence();
+    static_for<0, NK>([&](auto kc) {
+      constexpr int k = decltype(kc)::value;
+      constexpr int col0 = (32 * KC + KS * k) / N * N;
+      float(&dd)[N / 2] = *reinterpret_cast<float(*)[N / 2]>(&d[col0 / 2]);
+      Wgmma<N>::tf32_rs(dd, ahi[k], bdesc + 2 * k + 8 * col0, 1);
+      Wgmma<N>::tf32_rs(dd, ahi[k], blo + 2 * k + 8 * col0, 1);
+      Wgmma<N>::tf32_rs(dd, alo[k], bdesc + 2 * k + 8 * col0, 1);
+    });
+  } else {
+    wgmma_fence();
+    static_for<0, NK>([&](auto kc) {
+      constexpr int k = decltype(kc)::value;
+      constexpr int col0 = (32 * KC + KS * k) / N * N;
+      float(&dd)[N / 2] = *reinterpret_cast<float(*)[N / 2]>(&d[col0 / 2]);
+      if constexpr (MODE == kModeF16x3) {
+        Wgmma<N>::f16_ss(dd, adesc + 2 * k, bdesc + 2 * k + 8 * col0, 1);
+        Wgmma<N>::f16_ss(dd, adesc + 2 * k, bdesc + 4 + 2 * k + 8 * col0, 1);
+        Wgmma<N>::f16_ss(dd, adesc + 4 + 2 * k, bdesc + 2 * k + 8 * col0, 1);
+      } else if constexpr (MODE == kModeF16) {
+        Wgmma<N>::f16_ss(dd, adesc + 2 * k, bdesc + 2 * k + 8 * col0, 1);
+      } else {
+        Wgmma<N>::tf32_ss(dd, adesc + 2 * k, bdesc + 2 * k + 8 * col0, 1);
+      }
+    });
+  }
+  wgmma_commit();
+}
+
+// kb = the k-block's index in its tile (tap * k_chunks + half): which half of the tap's 64 channels it holds
+template <int MODE, int GW>
+__device__ __forceinline__ void mma_kblock_grouped(float (&d)[32], uint32_t a_addr, uint32_t b_addr, uint32_t b_lo_addr,
+                                                   const int wtid, const int kb) {
+  if (mode_bk(MODE) == 64 || (kb & 1) == 0) mma_kblock_grouped<MODE, GW, 0>(d, a_addr, b_addr, b_lo_addr, wtid);
+  else mma_kblock_grouped<MODE, GW, 1>(d, a_addr, b_addr, b_lo_addr, wtid);
+}
+
 struct MmaState {
   int stage;
   uint32_t phase;
@@ -283,10 +365,11 @@ struct MmaState {
 // Ring slots: hpc == 0: consecutive chunks alternate over the slots (conv_gemm: every reader of a slot reads all its chunks);
 // hpc > 0: the chunk of columns [32 c, 32 c + 32) goes to slot (c / hpc) & 1, the slot of the epilogue half that finishes
 // those columns in a chain layer (hpc = 32-column chunks per epilogue chunk).
-template <int PN, int STAGES, int MODE, class L>
+template <int PN, int STAGES, int MODE, class L, int GW = 0>
 __device__ __forceinline__ void mma_pass(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, uint64_t* split_bar,
                                          uint8_t* ring, uint64_t* ring_full, uint64_t* ring_empty, MmaState& ms, int kb0,
                                          int kb1, int seg_len, int wg, int wtid, int hpc) {
+  static_assert(GW == 0 || PN == 64, "grouped k-blocks need a 64-column pass");
   constexpr bool SPLIT3 = MODE == kModeSplit3;
   constexpr bool SEG = SPLIT3 || MODE == kModeF16x3;
   const int lane = wtid & 31;
@@ -296,10 +379,18 @@ __device__ __forceinline__ void mma_pass(uint8_t* smem, uint64_t* full_bar, uint
   for (int s0 = kb0, s1 = 0; s0 < kb1; s0 = s1) {
     s1 = (kb1 - s0 > seg_len) ? s0 + seg_len : kb1;
     int pending = -1;                            // stage whose MMAs may still be in flight
+    if constexpr (GW > 0) {
+#pragma unroll
+      for (int i = 0; i < PN / 2; ++i) d[i] = 0.f;
+    }
     for (int kb = s0; kb < s1; ++kb) {
       mbar_wait(SPLIT3 ? &split_bar[ms.stage] : &full_bar[ms.stage], ms.phase);
       const uint32_t a_addr = smem_u32(smem + ms.stage * L::kStageBytes);
-      mma_kblock<PN, MODE>(d, a_addr + wg * 64 * 128, a_addr + L::kABytes, a_addr + L::kABytes + L::kBBytes, wtid, kb == s0);
+      if constexpr (GW > 0)
+        mma_kblock_grouped<MODE, GW>(d, a_addr + wg * 64 * 128, a_addr + L::kABytes, a_addr + L::kABytes + L::kBBytes, wtid,
+                                     kb);
+      else
+        mma_kblock<PN, MODE>(d, a_addr + wg * 64 * 128, a_addr + L::kABytes, a_addr + L::kABytes + L::kBBytes, wtid, kb == s0);
       // SPLIT3 reads its A fragments into registers for every k-block: nothing stays in flight across them
       if (SPLIT3) wgmma_wait<0>(); else wgmma_wait<1>();
       if (pending >= 0) {
@@ -349,7 +440,7 @@ __device__ __forceinline__ void mma_pass(uint8_t* smem, uint64_t* full_bar, uint
 // swizzle row of halves) instead of 32.
 // Programmatic dependent launch: the prologue (barrier init, descriptor prefetch) runs before griddepcontrol.wait, i.e.
 // overlapped with the tail of the previous kernel on the stream; nothing before the wait touches global memory.
-template <int BN, int STAGES, int MODE, bool OUT16>
+template <int BN, int STAGES, int MODE, bool OUT16, int GW = 0>
 __global__ void __launch_bounds__(conv_gemm_threads(MODE), 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes,
@@ -470,8 +561,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     int t;
     int kb0, kb1;
     while (it.next(t, kb0, kb1)) {
-      mma_pass<P0, STAGES, MODE, L>(smem, full_bar, empty_bar, split_bar, ring, ring_full, ring_empty, ms, kb0, kb1, kSegLen,
-                                    wg, wtid, 0);
+      mma_pass<P0, STAGES, MODE, L, GW>(smem, full_bar, empty_bar, split_bar, ring, ring_full, ring_empty, ms, kb0, kb1,
+                                        kSegLen, wg, wtid, 0);
       if constexpr (P1 > 0)
         mma_pass<P1, STAGES, MODE, L>(smem, full_bar, empty_bar, split_bar, ring, ring_full, ring_empty, ms, kb0, kb1,
                                       kSegLen, wg, wtid, 0);
@@ -909,13 +1000,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 // ------------------------------------------------------------------ launch
 // pdl != 0: launched with programmatic stream serialization, i.e. this kernel's prologue may start while the
 // previous kernel on the stream drains (the kernel itself orders its memory accesses with griddepcontrol.wait).
-template <int BN, int STAGES, int MODE, bool OUT16>
+template <int BN, int STAGES, int MODE, bool OUT16, int GW = 0>
 static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
                       const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid, cudaStream_t stream, int pdl) {
   using L = SmemLayout<BN, STAGES, MODE>;
   static bool configured = false;
   if (!configured) {
-    MEGA_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_kernel<BN, STAGES, MODE, OUT16>,
+    MEGA_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_kernel<BN, STAGES, MODE, OUT16, GW>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
     configured = true;
   }
@@ -929,14 +1020,32 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUte
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl ? 1 : 0;
-  MEGA_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, STAGES, MODE, OUT16>, tmA, tmB, tmOut, tmRes, p));
+  MEGA_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, STAGES, MODE, OUT16, GW>, tmA, tmB, tmOut, tmRes, p));
   return MEGA_OK;
+}
+
+// the instantiation of a grouped launch's group width (block_n 64)
+template <int STAGES, int MODE, bool OUT16>
+static int launch_grouped(int gw, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
+                          const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid, cudaStream_t stream, int pdl) {
+  switch (gw) {
+    case 8: return launch_cfg<64, STAGES, MODE, OUT16, 8>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    case 16: return launch_cfg<64, STAGES, MODE, OUT16, 16>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    default: return launch_cfg<64, STAGES, MODE, OUT16, 32>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+  }
 }
 
 // fp16-operand instantiations live in their own translation unit (conv_gemm_f16.cu)
 int launch_conv_gemm_f16(int block_n, int out_f16, const CUtensorMap& tmA, const CUtensorMap& tmB,
                          const CUtensorMap& tmOut, const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid,
                          cudaStream_t stream, int pdl);
+
+// grouped launches (group width gw = 8 / 16 / 32, block_n 64) of the fp16 / split-fp16 modes
+int launch_conv_gemm_f16_grouped(int gw, int out_f16, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
+                                 const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid, cudaStream_t stream, int pdl);
+int launch_conv_gemm_f16x3_grouped(int gw, int out_split, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                                   const CUtensorMap& tmOut, const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid,
+                                   cudaStream_t stream, int pdl);
 
 // split-fp16 ("3xFP16") instantiations: conv_gemm_f16x3.cu
 int launch_conv_gemm_f16x3(int block_n, int out_split, const CUtensorMap& tmA, const CUtensorMap& tmB,

@@ -55,7 +55,7 @@ class ConvGemmDesc(ctypes.Structure):
         ("pdl", c_int),
         ("stride_h", c_int), ("stride_w", c_int), ("pad_w_set", c_int), ("pad_w", c_int),
         ("out_stride_h", c_ll), ("out_stride_n", c_ll), ("res_stride_h", c_ll), ("res_stride_n", c_ll),
-        ("b_lo_tap_off", c_int), ("res_split", c_int), ("acc_scale", ctypes.c_float), ("reserved_v6", c_int),
+        ("b_lo_tap_off", c_int), ("res_split", c_int), ("acc_scale", ctypes.c_float), ("group_width", c_int),
     ]
 
 

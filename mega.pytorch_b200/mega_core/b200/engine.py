@@ -144,7 +144,10 @@ class ResNetStages:
                 blk = _Block()
                 blk.w1 = pack_conv(sd[p + "conv1.weight"], dev, dtype)
                 blk.s1, blk.b1 = fold_bn(sd, p + "bn1.", dev)
-                blk.w2 = pack_conv(sd[p + "conv2.weight"], dev, dtype)
+                w2 = sd[p + "conv2.weight"]
+                blk.groups = sd[p + "conv1.weight"].shape[0] // w2.shape[1]     # ResNeXt: conv2 is grouped
+                blk.w2 = (pack_conv(w2, dev, dtype) if blk.groups == 1
+                          else ops.pack_grouped_conv(w2.float(), blk.groups, dev, dtype))
                 blk.s2, blk.b2 = fold_bn(sd, p + "bn2.", dev)
                 blk.w3 = pack_conv(sd[p + "conv3.weight"], dev, dtype)
                 blk.s3, blk.b3 = fold_bn(sd, p + "bn3.", dev)
@@ -225,8 +228,10 @@ class ResNetStages:
                 t1 = self._buf("t1", (n, ho, wo, blk.mid))
                 t2 = self._buf("t2", (n, ho, wo, blk.mid))
                 ops.conv_gemm(xs, blk.w1, t1, scale=blk.s1, bias=blk.b1, relu=True, max_ctas=max_ctas)
+                # a grouped conv2 goes in as its batched launch (the fields spelled out, not groups=: stand-ins for
+                # conv_gemm that know batched launches serve it unchanged)
                 ops.conv_gemm(t1, blk.w2, t2, taps=(3, 3), dil=blk.dil, pad=blk.dil, scale=blk.s2, bias=blk.b2,
-                              relu=True, max_ctas=max_ctas)
+                              relu=True, max_ctas=max_ctas, **(ops.grouped_fields(blk.w2) if blk.groups > 1 else {}))
                 if blk.wd is not None:
                     idn = self._buf("idn", (n, ho, wo, blk.cout))
                     ops.conv_gemm(xs, blk.wd, idn, scale=blk.sd, bias=blk.bd, relu=False, max_ctas=max_ctas)

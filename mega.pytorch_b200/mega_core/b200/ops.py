@@ -342,13 +342,17 @@ def pack_weights_split16(w, scale=None):
     normal fp16 numbers); conv_gemm multiplies the accumulator by 2^-e (exact). scale [rows]: a per-output-channel factor
     (FrozenBatchNorm) folded into the weights first -- the precision-3 kernel adds a bias only."""
     assert w.dtype == torch.float32 and w.dim() in (2, 3) and w.shape[-1] % 32 == 0
+    w0 = w
     if scale is not None:
         w = w * scale.to(w.device).float().view(-1, 1)
     m = float(w.abs().max())
     e = 0 if m == 0.0 else 13 - int(math.floor(math.log2(m)))
     e = max(-24, min(e, 40))
+    gw = _grouped_width(w0)
     out = split16_encode(w * (2.0 ** e))
     _SPLIT16_W[out.data_ptr()] = (weakref.ref(out), 2.0 ** -e)
+    if gw is not None:
+        _GROUPED_W[out.data_ptr()] = (weakref.ref(out), gw)
     return out
 
 
@@ -504,10 +508,53 @@ def pick_block_n(cout, m_tiles=0, batch=1):
     return pick_config(cout, max(m_tiles, 1), batch, 1)[0]
 
 
+# ---- grouped convolutions (ResNeXt conv2, MODEL.RESNETS.NUM_GROUPS > 1). The channels are cut into chunks of
+#      GROUP_CHUNK; chunk z runs as entry z of a channel-offset batched launch whose weight is the [taps, 64, 64] slice
+#      z of a block-diagonal [taps, C, 64] tensor: the gw x gw diagonal blocks hold the real weights, the rest is zero.
+GROUP_CHUNK = 64
+GROUP_WIDTHS = (8, 16, 32, 64)
+GROUP_DIAG = [True]     # grouped launches issue the MMAs of the diagonal blocks only (False: of the whole chunk; same result)
+_GROUPED_W = {}
+
+
+def _grouped_width(w):
+    r = _GROUPED_W.get(w.data_ptr())
+    if r is None:
+        return None
+    if r[0]() is None:
+        del _GROUPED_W[w.data_ptr()]
+        return None
+    return r[1]
+
+
+def pack_grouped_conv(w, groups, dev, dtype=torch.float32):
+    """grouped conv weight [C, C / groups, kh, kw] -> block-diagonal [kh*kw, C, GROUP_CHUNK] (row co = output channel,
+    column j = input channel GROUP_CHUNK * (co // GROUP_CHUNK) + j); pack_weights_split16 takes the result as it is"""
+    c, gw, kh, kw = w.shape
+    assert c == gw * groups and gw in GROUP_WIDTHS and c % GROUP_CHUNK == 0, \
+        "grouped conv: %d channels in %d groups (group width must be one of %s, channels a multiple of %d)" % (
+            c, groups, GROUP_WIDTHS, GROUP_CHUNK)
+    taps = w.permute(2, 3, 0, 1).reshape(kh * kw, c, gw)
+    out = torch.zeros(kh * kw, c, GROUP_CHUNK, dtype=w.dtype, device=w.device)
+    col = torch.arange(c, device=w.device) % GROUP_CHUNK // gw * gw        # first input column of each row's group
+    idx = (col.view(1, c, 1) + torch.arange(gw, device=w.device).view(1, 1, gw)).expand(kh * kw, c, gw)
+    out.scatter_(2, idx, taps)
+    out = out.contiguous().to(dev).to(dtype)
+    _GROUPED_W[out.data_ptr()] = (weakref.ref(out), gw)        # conv_gemm sets the launch's group_width from it
+    return out
+
+
+def grouped_fields(w):
+    """conv_gemm keyword arguments that run the packed weight `w` (pack_grouped_conv) as its channel-offset batched
+    launch: one batch entry per GROUP_CHUNK channels of input, weight rows, bias / scale, output and residual"""
+    c, z = w.shape[1], GROUP_CHUNK
+    return dict(batch=c // z, cout=z, k=z, block_n=z, a_c_off=z, b_n_off=z, out_c_off=z, res_c_off=z, bias_z_off=z)
+
+
 def conv_gemm(a, w, out, *, taps=(1, 1), dil=1, pad=0, scale=None, bias=None, residual=None,
               relu=False, tile=None, block_n=None, cout=None, k=None, batch=1, a_c_off=0,
               a_n_off=0, b_k_off=0, b_n_off=0, out_c_off=0, out_n_off=0, res_c_off=0, res_n_off=0, bias_z_off=0,
-              max_ctas=0, stream_k=None, out_hw=None, n_img=None, stride=(1, 1), pad_w=None):
+              max_ctas=0, stream_k=None, out_hw=None, n_img=None, stride=(1, 1), pad_w=None, groups=1):
     """out[n,h,w,:] = act(scale * conv(a, w) + bias + residual)   (wgmma tensor cores, fp32 accumulate)
 
     a   : [N,H,W,C] fp32 or fp16 view (innermost stride 1; other strides multiples of 16 bytes)
@@ -517,7 +564,15 @@ def conv_gemm(a, w, out, *, taps=(1, 1), dil=1, pad=0, scale=None, bias=None, re
     relu: False / True / "leaky" (LeakyReLU 0.1). stride = (stride_h, stride_w) of the convolution; pad_w: left padding
     when it differs from `pad` (rows). `out` (and `residual`) may be strided views in w / h / n (e.g. every other
     pixel of a larger map).
+    groups > 1: a grouped convolution whose weight was packed by pack_grouped_conv (the batched fields are implied).
     """
+    if groups > 1:
+        assert batch == 1 and cout is None and k is None and block_n is None and w.shape[2] == GROUP_CHUNK, \
+            "conv_gemm(groups=...): pass the weight from pack_grouped_conv and no batched fields"
+        g = grouped_fields(w)
+        return conv_gemm(a, w, out, taps=taps, dil=dil, pad=pad, scale=scale, bias=bias, residual=residual, relu=relu,
+                         tile=tile, max_ctas=max_ctas, stream_k=stream_k, out_hw=out_hw, n_img=n_img, stride=stride,
+                         pad_w=pad_w, **g)
     require_cuda(a, w, out, scale, bias, residual)
     f16 = a.dtype == torch.float16
     assert a.dtype == w.dtype and a.dtype in (torch.float32, torch.float16), (a.dtype, w.dtype)
@@ -591,6 +646,10 @@ def conv_gemm(a, w, out, *, taps=(1, 1), dil=1, pad=0, scale=None, bias=None, re
     d.a_c_off, d.a_n_off, d.b_k_off, d.b_n_off = a_c_off, a_n_off, b_k_off, b_n_off
     d.out_c_off, d.out_n_off, d.res_c_off, d.res_n_off = out_c_off, out_n_off, res_c_off, res_n_off
     d.bias_z_off = bias_z_off
+    gw = _grouped_width(w)
+    if (gw is not None and GROUP_DIAG[0] and batch > 1 and d.cout == d.k_per_tap == d.block_n == GROUP_CHUNK
+            and a_c_off == b_n_off == out_c_off == GROUP_CHUNK and b_k_off == 0):
+        d.group_width = gw
     d.max_ctas = max_ctas
     if SM_LIMIT[0] > 0:
         d.max_ctas = min(max_ctas, SM_LIMIT[0]) if max_ctas > 0 else SM_LIMIT[0]

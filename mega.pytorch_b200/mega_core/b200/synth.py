@@ -52,7 +52,7 @@ def _bn(sd, p, n, gen, out_scale=1.0, in_var=1.0):
     sd[p + "running_var"] = (torch.rand(n, generator=gen) * 0.2 + 0.9) * in_var
 
 
-def _stage(sd, prefix, gen, cin, mid, cout, blocks):
+def _stage(sd, prefix, gen, cin, mid, cout, blocks, groups=1):
     for b in range(blocks):
         p = prefix + "%d." % b
         if b == 0:
@@ -60,7 +60,7 @@ def _stage(sd, prefix, gen, cin, mid, cout, blocks):
             _bn(sd, p + "downsample.1.", cout, gen)
         sd[p + "conv1.weight"] = _kaiming((mid, cin if b == 0 else cout, 1, 1), gen)
         _bn(sd, p + "bn1.", mid, gen)
-        sd[p + "conv2.weight"] = _kaiming((mid, mid, 3, 3), gen)
+        sd[p + "conv2.weight"] = _kaiming((mid, mid // groups, 3, 3), gen)
         _bn(sd, p + "bn2.", mid, gen)
         sd[p + "conv3.weight"] = _kaiming((cout, mid, 1, 1), gen)
         _bn(sd, p + "bn3.", cout, gen, out_scale=0.25)   # damp the residual branch
@@ -75,22 +75,24 @@ def _linear(sd, p, nout, nin, gen, std=None, gain=1.0):
 
 def make_state_dict(arch="mega_r101", seed=0, num_classes=31):
     """state_dict with the reference's key names/shapes for
-    arch in {"mega_r101", "mega_r50", "rdn_r101", "fgfa_r101", "dff_r101", "base_r50", "base_r101"} (+ "_tiny" suffix: 1 block per stage,
-    for fast CPU tests)."""
+    arch in {"mega_r101", "mega_r50", "rdn_r101", "fgfa_r101", "dff_r101", "base_r50", "base_r101", "mega_x101", "base_x101"}
+    (+ "_tiny" suffix: 1 block per stage, for fast CPU tests). x101: ResNeXt-101 32x8d (NUM_GROUPS 32, WIDTH_PER_GROUP 8:
+    bottleneck widths 256 .. 2048, grouped conv2)."""
     gen = torch.Generator().manual_seed(seed)
     tiny = arch.endswith("_tiny")
     base = arch.replace("_tiny", "")
     method, depth = base.split("_")
-    blocks = {"r50": (3, 4, 6, 3), "r101": (3, 4, 23, 3)}[depth]
+    blocks = {"r50": (3, 4, 6, 3), "r101": (3, 4, 23, 3), "x101": (3, 4, 23, 3)}[depth]
+    groups, width = (32, 256) if depth == "x101" else (1, 64)      # res2 bottleneck width = NUM_GROUPS * WIDTH_PER_GROUP
     if tiny:
         blocks = (1, 1, 2, 1)
     sd = {}
     # stem: input std ~ 50 (0-255 domain); conv output variance ~ 2 * E[x^2]
     sd["backbone.body.stem.conv1.weight"] = _kaiming((64, 3, 7, 7), gen)
     _bn(sd, "backbone.body.stem.bn1.", 64, gen, in_var=2.0 * 70.0 ** 2)
-    c = _stage(sd, "backbone.body.layer1.", gen, 64, 64, 256, blocks[0])
-    c = _stage(sd, "backbone.body.layer2.", gen, c, 128, 512, blocks[1])
-    c = _stage(sd, "backbone.body.layer3.", gen, c, 256, 1024, blocks[2])
+    c = _stage(sd, "backbone.body.layer1.", gen, 64, width, 256, blocks[0], groups)
+    c = _stage(sd, "backbone.body.layer2.", gen, c, 2 * width, 512, blocks[1], groups)
+    c = _stage(sd, "backbone.body.layer3.", gen, c, 4 * width, 1024, blocks[2], groups)
     sd["rpn.anchor_generator.cell_anchors.0"] = None  # filled by the module / oracle (12 x 4)
     sd["rpn.head.conv.weight"] = _kaiming((1024, 1024, 3, 3), gen, gain=1.0)
     sd["rpn.head.conv.bias"] = torch.zeros(1024)
@@ -99,7 +101,7 @@ def make_state_dict(arch="mega_r101", seed=0, num_classes=31):
     sd["rpn.head.bbox_pred.weight"] = torch.randn(48, 1024, 1, 1, generator=gen) * (0.25 / 32)
     sd["rpn.head.bbox_pred.bias"] = torch.zeros(48)
     fe = "roi_heads.box.feature_extractor."
-    _stage(sd, fe + "head.layer4.", gen, 1024, 512, 2048, blocks[3])
+    _stage(sd, fe + "head.layer4.", gen, 1024, 8 * width, 2048, blocks[3], groups)
     if method == "base":
         sd[fe + "conv.weight"] = _kaiming((256, 2048, 1, 1), gen, gain=1.0)
         sd[fe + "conv.bias"] = torch.zeros(256)

@@ -13,9 +13,10 @@ def build_detection_model(cfg):
     return _DETECTION_META_ARCHITECTURES[cfg.MODEL.META_ARCHITECTURE](cfg)
 
 
-def vid_config(method="mega", conv_body="R-101-C4", device="cuda"):
+def vid_config(method="mega", conv_body="R-101-C4", device="cuda", num_groups=1, width_per_group=64):
     """the configuration tools/test_net.py ends up with for the VID configs: defaults <- BASE_RCNN_1gpu.yaml
-    <- configs/MEGA/vid_R_101_C4_MEGA_1x.yaml (or configs/vid_R_50_C4_1x.yaml for method="base")"""
+    <- configs/MEGA/vid_R_101_C4_MEGA_1x.yaml (or configs/vid_R_50_C4_1x.yaml for method="base");
+    num_groups / width_per_group: MODEL.RESNETS.NUM_GROUPS / WIDTH_PER_GROUP (32 / 8 for a ResNeXt-101 32x8d body)"""
     from ...config import cfg as base
     c = base.clone()
     c.merge_from_dict({
@@ -23,7 +24,8 @@ def vid_config(method="mega", conv_body="R-101-C4", device="cuda"):
                   "RPN": {"ANCHOR_SIZES": (64, 128, 256, 512), "PRE_NMS_TOP_N_TEST": 6000, "POST_NMS_TOP_N_TEST": 300},
                   "ROI_HEADS": {"SCORE_THRESH": 0.001, "NMS": 0.5, "DETECTIONS_PER_IMG": 300},
                   "ROI_BOX_HEAD": {"NUM_CLASSES": 31, "POOLER_RESOLUTION": 7, "PREDICTOR": "FPNPredictor"},
-                  "RESNETS": {"RES5_DILATION": 2}, "BACKBONE": {"CONV_BODY": conv_body}},
+                  "RESNETS": {"RES5_DILATION": 2, "NUM_GROUPS": num_groups, "WIDTH_PER_GROUP": width_per_group},
+                  "BACKBONE": {"CONV_BODY": conv_body}},
         "INPUT": {"MIN_SIZE_TEST": 600, "MAX_SIZE_TEST": 1000}, "TEST": {"IMS_PER_BATCH": 1, "DETECTIONS_PER_IMG": 300}})
     if method == "mega":
         c.merge_from_dict({"MODEL": {"META_ARCHITECTURE": "GeneralizedRCNNMEGA",
@@ -50,12 +52,15 @@ def vid_config(method="mega", conv_body="R-101-C4", device="cuda"):
 
 
 def build_detection_model_from_state_dict(sd, method="mega", device="cuda", precision=None):
-    """convenience for benchmarks/tests: infer the conv body from the state dict, build, load, eval"""
+    """convenience for benchmarks/tests: infer the conv body (depth, ResNeXt groups and width) from the state dict,
+    build, load, eval"""
     n3 = 0
     while ("backbone.body.layer3.%d.conv1.weight" % n3) in sd:
         n3 += 1
     body = {6: "R-50-C4", 23: "R-101-C4"}.get(n3)
-    cfg = vid_config(method, body or "R-101-C4", device)
+    w2 = sd["backbone.body.layer1.0.conv2.weight"]              # [G * width, width, 3, 3]
+    cfg = vid_config(method, body or "R-101-C4", device, num_groups=w2.shape[0] // w2.shape[1],
+                     width_per_group=w2.shape[1])
     if precision is not None:
         cfg.MODEL.B200.PRECISION = precision
     if method == "base" and "roi_heads.box.feature_extractor.conv.weight" not in sd:

@@ -48,24 +48,30 @@ def _image_size(images):
 
 
 class Bottleneck(nn.Module):
-    def __init__(self, cin, mid, cout, stride, dilation):
+    def __init__(self, cin, mid, cout, stride, dilation, groups=1):
         super().__init__()
         if cin != cout:
             self.downsample = nn.Sequential(Conv2d(cin, cout, 1, stride=(stride if dilation == 1 else 1), bias=False),
                                             FrozenBatchNorm2d(cout))
         self.conv1 = Conv2d(cin, mid, 1, stride=(1 if dilation > 1 else stride), bias=False)
         self.bn1 = FrozenBatchNorm2d(mid)
-        self.conv2 = Conv2d(mid, mid, 3, padding=dilation, dilation=dilation, bias=False)
+        self.conv2 = Conv2d(mid, mid, 3, padding=dilation, dilation=dilation, groups=groups, bias=False)
         self.bn2 = FrozenBatchNorm2d(mid)
         self.conv3 = Conv2d(mid, cout, 1, bias=False)
         self.bn3 = FrozenBatchNorm2d(cout)
 
 
-def _stage(cin, mid, cout, n, stride, dilation=1):
+def _stage(cin, mid, cout, n, stride, dilation=1, groups=1):
     blocks = []
     for i in range(n):
-        blocks.append(Bottleneck(cin if i == 0 else cout, mid, cout, stride if i == 0 else 1, dilation))
+        blocks.append(Bottleneck(cin if i == 0 else cout, mid, cout, stride if i == 0 else 1, dilation, groups))
     return nn.Sequential(*blocks)
+
+
+def bottleneck_width(cfg, stage):
+    """conv1 / conv2 width of res`stage+1` (resnet.py:98-108): NUM_GROUPS * WIDTH_PER_GROUP * 2^(stage-1)"""
+    r = cfg.MODEL.RESNETS
+    return r.NUM_GROUPS * r.WIDTH_PER_GROUP * 2 ** (stage - 1)
 
 
 class Stem(nn.Module):
@@ -78,22 +84,24 @@ class Stem(nn.Module):
 class ResNetBody(nn.Module):
     """`backbone.body` (modeling/backbone/resnet.py:81-152)"""
 
-    def __init__(self, conv_body):
+    def __init__(self, cfg):
         super().__init__()
-        b = BLOCKS[conv_body]
+        b = BLOCKS[cfg.MODEL.BACKBONE.CONV_BODY]
+        g = cfg.MODEL.RESNETS.NUM_GROUPS
         self.stem = Stem()
-        self.layer1 = _stage(64, 64, 256, b[0], 1)
-        self.layer2 = _stage(256, 128, 512, b[1], 2)
-        self.layer3 = _stage(512, 256, 1024, b[2], 2)
+        self.layer1 = _stage(64, bottleneck_width(cfg, 1), 256, b[0], 1, groups=g)
+        self.layer2 = _stage(256, bottleneck_width(cfg, 2), 512, b[1], 2, groups=g)
+        self.layer3 = _stage(512, bottleneck_width(cfg, 3), 1024, b[2], 2, groups=g)
         self.out_channels = 1024
 
 
 class ResNetHead(nn.Module):
     """res5 as `feature_extractor.head` (resnet.py:155-204; stride_init=1)"""
 
-    def __init__(self, dilation):
+    def __init__(self, cfg):
         super().__init__()
-        self.layer4 = _stage(1024, 512, 2048, 3, 1, dilation)
+        self.layer4 = _stage(1024, bottleneck_width(cfg, 4), 2048, 3, 1, cfg.MODEL.RESNETS.RES5_DILATION,
+                             cfg.MODEL.RESNETS.NUM_GROUPS)
         self.out_channels = 2048
 
 
@@ -114,7 +122,7 @@ class _Backbone(nn.Sequential, _EngineServed):
 @registry.BACKBONES.register("R-101-C4")
 def build_resnet_backbone(cfg):
     model = _Backbone()
-    model.add_module("body", ResNetBody(cfg.MODEL.BACKBONE.CONV_BODY))
+    model.add_module("body", ResNetBody(cfg))
     model.out_channels = cfg.MODEL.RESNETS.BACKBONE_OUT_CHANNELS
     return model
 
@@ -182,7 +190,7 @@ def _fc(i, o):
 class ResNetConv52MLPFeatureExtractor(nn.Module):
     def __init__(self, cfg, in_channels):
         super().__init__()
-        self.head = ResNetHead(cfg.MODEL.RESNETS.RES5_DILATION)
+        self.head = ResNetHead(cfg)
         ch = 2048
         if cfg.MODEL.VID.ROI_BOX_HEAD.REDUCE_CHANNEL:
             self.conv = nn.Conv2d(2048, 256, 1)
@@ -228,7 +236,7 @@ class MEGAFeatureExtractor(_WindowedExtractorForward, nn.Module):
 
     def __init__(self, cfg, in_channels):
         super().__init__()
-        self.head = ResNetHead(cfg.MODEL.RESNETS.RES5_DILATION)
+        self.head = ResNetHead(cfg)
         self.conv = None
         res = cfg.MODEL.ROI_BOX_HEAD.POOLER_RESOLUTION
         dim = cfg.MODEL.ROI_BOX_HEAD.MLP_HEAD_DIM
@@ -254,7 +262,7 @@ class RDNFeatureExtractor(_WindowedExtractorForward, nn.Module):
 
     def __init__(self, cfg, in_channels):
         super().__init__()
-        self.head = ResNetHead(cfg.MODEL.RESNETS.RES5_DILATION)
+        self.head = ResNetHead(cfg)
         self.conv = None
         res = cfg.MODEL.ROI_BOX_HEAD.POOLER_RESOLUTION
         dim = cfg.MODEL.ROI_BOX_HEAD.MLP_HEAD_DIM
@@ -361,6 +369,17 @@ def engine_config_from(cfg):
     if v.METHOD in ("rdn", "mega") and v.RPN.REF_PRE_NMS_TOP_N != m.RPN.PRE_NMS_TOP_N_TEST:
         unsupported.append("MODEL.VID.RPN.REF_PRE_NMS_TOP_N != MODEL.RPN.PRE_NMS_TOP_N_TEST (the reference proposals of a frame "
                            "are taken as the prefix of its key proposals, which needs equal pre-NMS sets)")
+    g, wpg = m.RESNETS.NUM_GROUPS, m.RESNETS.WIDTH_PER_GROUP
+    for stage in (1, 2, 3, 4):
+        width, gw = g * wpg * 2 ** (stage - 1), wpg * 2 ** (stage - 1)
+        if width % 64 or (g > 1 and gw not in (8, 16, 32, 64)):
+            unsupported.append("MODEL.RESNETS.NUM_GROUPS = %d / WIDTH_PER_GROUP = %d (res%d: bottleneck width %d, group "
+                               "width %d; the kernels serve widths in multiples of 64 and group widths 8, 16, 32 or 64)"
+                               % (g, wpg, stage + 1, width, gw))
+            break
+    if any(m.RESNETS.STAGE_WITH_DCN):
+        unsupported.append("MODEL.RESNETS.STAGE_WITH_DCN = %s (the engines have no deformable backbone stages)"
+                           % (tuple(m.RESNETS.STAGE_WITH_DCN),))
     if v.METHOD == "mega":
         if not (v.MEGA.MEMORY.ENABLE and v.MEGA.GLOBAL.ENABLE):
             unsupported.append("MODEL.VID.MEGA.MEMORY.ENABLE / GLOBAL.ENABLE = False (MegaEngine is laid out for memory + "
