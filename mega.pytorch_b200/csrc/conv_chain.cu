@@ -74,11 +74,6 @@ __device__ __forceinline__ void grid_wait(const unsigned* ctr, unsigned target) 
   fence_proxy_async_all();
 }
 
-struct PipeState {
-  int stage;
-  uint32_t phase;
-};
-
 // optional in-kernel event trace of ONE CTA (diagnostics): (tag, SM clock) pairs per role
 struct ChainTrace {
   unsigned long long* buf;   // [3 roles][kTraceCap][2] or NULL
@@ -125,7 +120,6 @@ constexpr int kChainEpiWarp0 = 8;
 constexpr int kChainProducerWarp = 16;
 constexpr int kChainThreads = (kChainProducerWarp + 1) * 32;
 
-__device__ __forceinline__ void epi_bar_sync_all() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   uint4 v;
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
@@ -246,60 +240,33 @@ __device__ __forceinline__ void chain_epilogue_layer(const ChainLayer* L, const 
   for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item) {
     const TileCoord tc = decode_tile(p, t, BN);
     const bool complete = (kb0 == 0 && kb1 == KB);
-    const int r0 = q * 32;
-    const int bh0 = r0 / p.tile_w, bw0 = r0 - bh0 * p.tile_w;
-    const int st_w = tc.w0 + bw0, st_h = tc.h0 + bh0;
-    const int res_n = tc.img + tc.batch * p.res_n_off;
+    const StoreBox box = store_box(p, tc, q);
     const int nchunks = min(BN / CW, (p.cout - tc.n0 + CW - 1) / CW);
     // ---- while the MMAs of this tile run: stage its scale / bias slice in shared memory and start this warp's first
     //      residual load
-    epi_bar_sync_all();   // every warp is done with the previous tile's scale / bias
-    if (epi_tid < BN) {
-      const int n = tc.n0 + epi_tid;
-      const int zoff = tc.batch * p.bias_z_off;
-      sb_s[epi_tid] = (p.scale && n < p.cout) ? __ldg(p.scale + zoff + n) : 1.f;
-      sb_s[128 + epi_tid] = (p.bias && n < p.cout) ? __ldg(p.bias + zoff + n) : 0.f;
-    }
+    epi_bar_sync<kEpiThreads>();   // every warp is done with the previous tile's scale / bias
+    if (epi_tid < BN) stage_scale_bias(sb_s, 128, p, tc, epi_tid);
     if (complete && has_res && lane == 0 && half < nchunks) {
       mbar_arrive_expect_tx(rbar, 4096);
       tma_load_4d(reinterpret_cast<void*>(smem + kChainEpiOffset + ew * 8192 + 4096), tmRes, rbar,
-                  tc.n0 + half * CW + tc.batch * p.res_c_off, st_w, st_h, res_n);
+                  tc.n0 + half * CW + tc.batch * p.res_c_off, box.w, box.h, box.res_n);
     }
-    epi_bar_sync_all();
+    epi_bar_sync<kEpiThreads>();
     tr.put(TR_TAG(layer, tile_item, 4));
     bool finalize = complete;
     int c_first = cta, c_last = cta;
     if (!complete) {
       // ---- publish this CTA's partial accumulator (each warp its own columns), then find out whether it arrived last
-      float* my_ws = p.part_ws + ((static_cast<long long>(cta) * 2 + (tile_item == 0 ? 0 : 1)) * kBM + row) * BN;
+      float* part = sk_own_part_row(p, cta, tile_item, row, BN);
       for (int c = half; c < BN / CW; c += 2) {
 #pragma unroll 1
         for (int h = 0; h < HPC; ++h) {
-          const int g32 = c * HPC + h;
           uint32_t acc[32];
           ring_take(ring, ring_full, ring_empty, half, ruse++, row, acc);
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 v = make_float4(__uint_as_float(acc[j]), __uint_as_float(acc[j + 1]), __uint_as_float(acc[j + 2]),
-                                   __uint_as_float(acc[j + 3]));
-            __stcg(reinterpret_cast<float4*>(my_ws + g32 * 32 + j), v);
-          }
+          sk_publish(part, (c * HPC + h) * 32, acc);
         }
       }
-      __threadfence();
-      epi_bar_sync_all();
-      c_first = unit_owner(U, grid, t * KB);
-      c_last = unit_owner(U, grid, t * KB + KB - 1);
-      if (epi_tid == 0) {
-        const int parts = c_last - c_first + 1;
-        const int old = atomicAdd(&p.counters[t], 1);
-        const int last = (old == parts - 1);
-        if (last) p.counters[t] = 0;
-        *epi_flag = last;
-      }
-      epi_bar_sync_all();
-      finalize = (*epi_flag != 0);
-      if (finalize) __threadfence();
+      finalize = sk_elect_finisher<kEpiThreads>(p, U, grid, KB, t, epi_tid, epi_flag, c_first, c_last);
     }
     if (finalize) {
       const int out_n = tc.img + tc.batch * p.out_n_off;
@@ -310,7 +277,7 @@ __device__ __forceinline__ void chain_epilogue_layer(const ChainLayer* L, const 
           if ((!complete || c != half) && lane == 0) {   // (whole tiles started their first load before the MMAs)
             mbar_arrive_expect_tx(rbar, 4096);
             tma_load_4d(reinterpret_cast<void*>(smem + kChainEpiOffset + ew * 8192 + 4096), tmRes, rbar,
-                        nb + tc.batch * p.res_c_off, st_w, st_h, res_n);
+                        nb + tc.batch * p.res_c_off, box.w, box.h, box.res_n);
           }
           mbar_wait(rbar, (rphase >> ew) & 1u);
           rphase ^= (1u << ew);
@@ -326,19 +293,8 @@ __device__ __forceinline__ void chain_epilogue_layer(const ChainLayer* L, const 
           if (complete) {
             ring_take(ring, ring_full, ring_empty, half, ruse++, row, raw);
           } else {
-            // deterministic reduction: parts summed in CTA order (this CTA's own part as published above)
             float sum[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) sum[j] = 0.f;
-            for (int oc = c_first; oc <= c_last; ++oc) {
-              const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
-              const float* ws = p.part_ws + ((static_cast<long long>(oc) * 2 + slot) * kBM + row) * BN + col0;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + j));
-                sum[j] += v.x; sum[j + 1] += v.y; sum[j + 2] += v.z; sum[j + 3] += v.w;
-              }
-            }
+            sk_reduce(p, U, grid, KB, t, c_first, c_last, row, BN, col0, sum);
 #pragma unroll
             for (int j = 0; j < 32; ++j) raw[j] = __float_as_uint(sum[j]);
           }
@@ -347,8 +303,7 @@ __device__ __forceinline__ void chain_epilogue_layer(const ChainLayer* L, const 
         fence_async_smem();
         __syncwarp();
         if (lane == 0) {
-          tma_store_4d(tmOut, smem + kChainEpiOffset + ew * 8192, nb + tc.batch * p.out_c_off, st_w, st_h,
-                       out_n);
+          tma_store_4d(tmOut, smem + kChainEpiOffset + ew * 8192, nb + tc.batch * p.out_c_off, box.w, box.h, out_n);
           tma_store_commit();
         }
       }
@@ -401,8 +356,6 @@ conv_chain_kernel(const ChainLayer* __restrict__ layers, const int n_layers, uns
 
   if (warp == kChainProducerWarp) {
     // ===================== TMA producer =====================
-    // lane 0 loads the A (activation) tile and posts the expected byte count, lane 1 loads the B (weight) tile: the two
-    // descriptor-based copies of a k-block are issued in parallel
     if (lane < 2) {
       PipeState ps = {0, 0};
       TraceCursor tr = trace_cursor(trace, 0, cta);
@@ -414,11 +367,6 @@ conv_chain_kernel(const ChainLayer* __restrict__ layers, const int n_layers, uns
         const ConvGemmParams p = L->p;
         const int BN = L->block_n;
         const int act = L->active_ctas;
-        const int k_chunks = p.k_chunks, taps_s = p.taps_s, dil = p.dil, pad = p.pad, pad_w = p.pad_w;
-        const int stride_h = p.stride_h, stride_w = p.stride_w;
-        const int a_c_off = p.a_c_off, a_n_off = p.a_n_off, b_k_off = p.b_k_off, b_n_off = p.b_n_off;
-        const CUtensorMap* tmA = &L->tmA;
-        const CUtensorMap* tmB = &L->tmB;
         const uint32_t tx_bytes = static_cast<uint32_t>((kBM + BN) * 128);
         tr.put(TR_TAG(l, 0, 1));
         // layer l may read what layers <= l - depth wrote: all CTAs have arrived l / depth times at counter l % depth
@@ -432,36 +380,8 @@ conv_chain_kernel(const ChainLayer* __restrict__ layers, const int n_layers, uns
         int kb0, kb1;
         while (it.next(t, kb0, kb1)) {
           const TileCoord tc = decode_tile(p, t, BN);
-          int tap = kb0 / k_chunks;
-          int kc = kb0 - tap * k_chunks;
-          int r = tap / taps_s;
-          int sx = tap - r * taps_s;
-          const int a_c0 = tc.batch * a_c_off, a_n = tc.img + tc.batch * a_n_off;
-          const int b_k0 = tc.batch * b_k_off, b_n = tc.n0 + tc.batch * b_n_off;
-          for (int kb = kb0; kb < kb1; ++kb) {
-            mbar_wait(&empty_bar[ps.stage], ps.phase ^ 1);
-            tr.put(TR_TAG(l, kb, 3));
-            uint8_t* a_dst = smem + ps.stage * kChainStageBytes;
-            if (lane == 0) {
-              mbar_arrive_expect_tx(&full_bar[ps.stage], tx_bytes);
-              tma_load_4d(a_dst, tmA, &full_bar[ps.stage], kc * 64 + a_c0, tc.w0 * stride_w + sx * dil - pad_w,
-                          tc.h0 * stride_h + r * dil - pad, a_n);
-            } else {
-              tma_load_3d(a_dst + kChainABytes, tmB, &full_bar[ps.stage], kc * 64 + b_k0, b_n, tap);
-            }
-            if (++kc == k_chunks) {
-              kc = 0;
-              ++tap;
-              if (++sx == taps_s) {
-                sx = 0;
-                ++r;
-              }
-            }
-            if (++ps.stage == kChainStages) {
-              ps.stage = 0;
-              ps.phase ^= 1;
-            }
-          }
+          produce_pass<kChainStages>(&L->tmA, &L->tmB, full_bar, empty_bar, ps, smem, kChainStageBytes, kChainABytes, 0, 64,
+                                     tx_bytes, p, tc, tc.n0, kb0, kb1, lane, [&](int kb) { tr.put(TR_TAG(l, kb, 3)); });
         }
       }
     }
@@ -516,7 +436,7 @@ conv_chain_kernel(const ChainLayer* __restrict__ layers, const int n_layers, uns
       // (one poller per CTA; the named barrier passes the acquired state on to the other epilogue threads)
       if (l >= depth) {
         if (epi_tid == 0) grid_wait(sync + (l % depth), static_cast<unsigned>(l / depth) * grid);
-        epi_bar_sync_all();
+        epi_bar_sync<kEpiThreads>();
         fence_proxy_async_all();
       }
       const ConvGemmParams p = L->p;
@@ -538,7 +458,7 @@ conv_chain_kernel(const ChainLayer* __restrict__ layers, const int n_layers, uns
       //  wait_group; the named barrier orders all of that before thread 0's single gpu-scope release)
       if (lane == 0) tma_store_wait<0>();
       tr.put(TR_TAG(l, 0, 9));
-      epi_bar_sync_all();
+      epi_bar_sync<kEpiThreads>();
       if (epi_tid == 0) {
         fence_proxy_async_all();
         __threadfence();

@@ -1,24 +1,9 @@
-// Implicit-GEMM convolution / GEMM on the Hopper tensor cores (wgmma, TF32 operands,
-// FP32 accumulate in registers), fed by TMA with the 128-byte shared-memory swizzle.
-//
-// One kernel serves every dense contraction of the MEGA hot path:
-//   * backbone / res5 / RPN-head convolutions (1x1, 3x3, 3x3 dilated) over NHWC maps
-//     (reference: mega_core/modeling/backbone/resnet.py:324-344, rpn/rpn.py:99-106),
-//     with FrozenBatchNorm scale/bias (layers/batch_norm.py:26-31), residual add and ReLU
-//     folded into the epilogue;
-//   * Linear layers (make_layers.py:80-92) as a 1x1 "convolution" over an H=1 image;
-//   * the per-head Q.K^T and P.V' products of the relation module
-//     (roi_box_feature_extractors.py:602-646) through the batch (grid.z) offsets.
-//
-// Tiling: the M tile is a th x tw rectangle of 128 output pixels, so the A operand of filter
-// tap (r,s) is the same rectangle shifted by (r,s)*dilation - pad: a plain 4-D tiled TMA load
-// with out-of-bounds zero fill supplies the padding. K is consumed in slabs of 32 floats
-// (= one 128 B swizzle row) per tap. Warp roles: warp 0 TMA producer, two MMA warpgroups,
-// warps 2-5 epilogue (accumulator ring -> registers -> global); the strict modes add warps 6-9: operand splitters (3xTF32)
-// or a second set of epilogue warps (3xFP16 on split-fp16 tensors, the mode the strict engine runs; see conv_gemm_kernel.cuh).
 #include "conv_gemm_kernel.cuh"
 
 namespace mega {
+
+template MEGA_LAUNCH_MODE(kModeTf32);
+template MEGA_LAUNCH_MODE(kModeSplit3);
 
 // ------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -327,36 +312,17 @@ extern "C" int mega_conv_gemm(const mega_conv_gemm_desc* d, void* stream_v) {
   int ctas = 0;
   const int erc = encode_conv_gemm_problem(d, &tmA, &tmB, &tmOut, &tmRes, &p, &ctas);
   if (erc != MEGA_OK) return erc;
-  const bool strict = d->precision == kModeSplit3;
-  const bool f16 = d->precision == kModeF16;
   const bool out16 = d->out_f16 != 0;
   dim3 grid(static_cast<unsigned>(ctas), 1, 1);
   const int pdl = d->pdl ? 1 : 0;
   // grouped launches (block_n 64, checked by the encoder) issue only the diagonal blocks; with one group per 64 channels
   // (gw 64) that is the dense k-block. The layer chain runs grouped layers with the dense issue (same result).
   const int gw = d->group_width == 64 ? 0 : d->group_width;
-  if (gw != 0) {
-    if (d->precision == kModeF16x3)
-      return launch_conv_gemm_f16x3_grouped(gw, out16 ? 1 : 0, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    if (f16) return launch_conv_gemm_f16_grouped(gw, out16 ? 1 : 0, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    if (strict) return launch_grouped<4, kModeSplit3, false>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    return launch_grouped<5, kModeTf32, false>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-  }
-  if (d->precision == kModeF16x3)
-    return launch_conv_gemm_f16x3(d->block_n, out16 ? 1 : 0, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-  if (f16) return launch_conv_gemm_f16(d->block_n, out16 ? 1 : 0, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-  if (strict) {
-    return d->block_n == 64 ? launch_cfg<64, 4, kModeSplit3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
-                            : launch_cfg<128, 2, kModeSplit3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-  }
-  switch (d->block_n) {
-    case 32: return launch_cfg<32, 6, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    case 64: return launch_cfg<64, 5, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    case 96: return launch_cfg<96, 4, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    case 128: return launch_cfg<128, 4, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    case 160: return launch_cfg<160, 3, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    case 192: return launch_cfg<192, 3, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    default: return launch_cfg<256, 2, kModeTf32, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+  switch (d->precision) {
+    case kModeTf32: return launch_mode<kModeTf32>(d->block_n, out16, gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    case kModeSplit3: return launch_mode<kModeSplit3>(d->block_n, out16, gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    case kModeF16: return launch_mode<kModeF16>(d->block_n, out16, gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    default: return launch_mode<kModeF16x3>(d->block_n, out16, gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
   }
 }
 

@@ -5,25 +5,6 @@
 
 namespace mega {
 
-int launch_conv_gemm_f16x3(int block_n, int out_split, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                           const CUtensorMap& tmOut, const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid,
-                           cudaStream_t stream, int pdl) {
-  if (block_n == 64) {
-    return out_split ? launch_cfg<64, 5, kModeF16x3, true>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
-                     : launch_cfg<64, 5, kModeF16x3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-  }
-  if (block_n == 128) {
-    return out_split ? launch_cfg<128, 4, kModeF16x3, true>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
-                     : launch_cfg<128, 4, kModeF16x3, false>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-  }
-  mega_set_error("conv_gemm: 3xfp16 supports block_n 64 / 128 (got %d)", block_n);
-  return MEGA_ERR_ARG;
-}
-
-int launch_conv_gemm_f16x3_grouped(int gw, int out_split, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
-                                   const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid, cudaStream_t stream, int pdl) {
-  return out_split ? launch_grouped<5, kModeF16x3, true>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl)
-                   : launch_grouped<5, kModeF16x3, false>(gw, tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-}
+template MEGA_LAUNCH_MODE(kModeF16x3);
 
 }  // namespace mega

@@ -51,6 +51,13 @@ __host__ __device__ constexpr int conv_gemm_threads(int mode) { return (mma_warp
 // An N tile wider than 128 columns is computed in two passes over the same k-blocks (columns [0, P0), then [P0, block_n)):
 // a pass keeps at most 64 accumulator registers per MMA thread. Both widths are multiples of 32 (whole ring chunks).
 __host__ __device__ constexpr int pass_n(int bn) { return bn <= 128 ? bn : (bn == 160 ? 96 : bn / 2); }
+// Pipeline stages of the (mode, block_n) kernel, grouped launches (block_n 64) included; conv_gemm_kernel checks that they
+// fit the 227 KB of shared memory next to the ring and the epilogue staging.
+constexpr int conv_gemm_stages(int mode, int bn) {
+  if (mode == kModeSplit3) return bn == 64 ? 4 : 2;
+  if (mode == kModeF16x3) return bn == 64 ? 5 : 4;
+  return bn == 32 ? 6 : bn == 64 ? 5 : bn <= 128 ? 4 : bn <= 192 ? 3 : 2;
+}
 
 struct ConvGemmParams {
   int tiles_w, tiles_h, tile_w, tile_h;
@@ -163,8 +170,143 @@ struct WorkIter {
   }
 };
 
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-__device__ __forceinline__ void epi_bar_sync8() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // 8 epilogue warps
+// named barrier of the THREADS epilogue threads
+template <int THREADS>
+__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(THREADS) : "memory"); }
+
+// ------------------------------------------------------------------ stream-K fix-up
+// A tile whose k-blocks straddle CTAs c_first .. c_last is finished by the last of them to arrive. Each publishes its partial
+// accumulator to part_ws[cta][slot][kBM][bn]. Only the first and the last work item of a CTA's unit range can be partial, so
+// two slots per CTA suffice: slot 0 holds the CTA's first item, slot 1 any later one. The finisher derives the slot of CTA
+// oc's part of tile t from where oc's range starts (inside t: t was its first item), and sums the parts in CTA order, so
+// the result does not depend on which CTA arrives last.
+__device__ __forceinline__ float* sk_part_row(const ConvGemmParams& p, int c, int slot, int row, int bn) {
+  return p.part_ws + ((static_cast<long long>(c) * 2 + slot) * kBM + row) * bn;
+}
+
+// tile row `row` of this CTA's part of its tile_item-th work item
+__device__ __forceinline__ float* sk_own_part_row(const ConvGemmParams& p, int cta, int tile_item, int row, int bn) {
+  return sk_part_row(p, cta, tile_item == 0 ? 0 : 1, row, bn);
+}
+
+// columns [col0, col0 + 32) of a row of this CTA's part (callers take `part` from sk_own_part_row once per item, before
+// they wait for their first chunk: computed after the wait, the address costs the 3xFP16 epilogue spills)
+__device__ __forceinline__ void sk_publish(float* part, int col0, const uint32_t (&acc)[32]) {
+  float* ws = part + col0;
+#pragma unroll
+  for (int j = 0; j < 32; j += 4)
+    __stcg(reinterpret_cast<float4*>(ws + j), make_float4(__uint_as_float(acc[j]), __uint_as_float(acc[j + 1]),
+                                                          __uint_as_float(acc[j + 2]), __uint_as_float(acc[j + 3])));
+}
+
+// Called by all THREADS epilogue threads once they have published their chunks of tile t. Counts this CTA's arrival; the
+// last of the c_first .. c_last arrivals resets the counter for the next launch. True in every thread of the finisher.
+template <int THREADS>
+__device__ __forceinline__ bool sk_elect_finisher(const ConvGemmParams& p, int U, int grid, int KB, int t, int epi_tid,
+                                                  int* flag, int& c_first, int& c_last) {
+  __threadfence();
+  epi_bar_sync<THREADS>();
+  c_first = unit_owner(U, grid, t * KB);
+  c_last = unit_owner(U, grid, t * KB + KB - 1);
+  if (epi_tid == 0) {
+    const int parts = c_last - c_first + 1;
+    const int old = atomicAdd(&p.counters[t], 1);
+    const int last = (old == parts - 1);
+    if (last) p.counters[t] = 0;
+    *flag = last;
+  }
+  epi_bar_sync<THREADS>();
+  const bool finisher = *flag != 0;
+  if (finisher) __threadfence();
+  return finisher;
+}
+
+// columns [col0, col0 + 32) of tile row `row` of tile t: the parts of CTAs c_first .. c_last summed in CTA order
+__device__ __forceinline__ void sk_reduce(const ConvGemmParams& p, int U, int grid, int KB, int t, int c_first, int c_last,
+                                          int row, int bn, int col0, float (&acc)[32]) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+  for (int oc = c_first; oc <= c_last; ++oc) {
+    const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
+    const float* ws = sk_part_row(p, oc, slot, row, bn) + col0;
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) {
+      const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + j));
+      acc[j] += v.x; acc[j + 1] += v.y; acc[j + 2] += v.z; acc[j + 3] += v.w;
+    }
+  }
+}
+
+// ------------------------------------------------------------------ epilogue staging
+// Origin of the store / residual box of the warps of 32-row quarter q (tile rows [32 q, 32 q + 32) = box_h x box_w output
+// pixels), and the residual's image index.
+struct StoreBox {
+  int w, h, res_n;
+};
+__device__ __forceinline__ StoreBox store_box(const ConvGemmParams& p, const TileCoord& tc, int q) {
+  const int r0 = q * 32;
+  const int bh0 = r0 / p.tile_w, bw0 = r0 - bh0 * p.tile_w;
+  return {tc.w0 + bw0, tc.h0 + bh0, tc.img + tc.batch * p.res_n_off};
+}
+
+// Column i of the tile's scale / bias slice into shared memory (scale at sb, bias at sb + bias_off), so that the chunk loops
+// read them with broadcast loads; columns past cout get scale 1 and bias 0.
+__device__ __forceinline__ void stage_scale_bias(float* sb, int bias_off, const ConvGemmParams& p, const TileCoord& tc, int i) {
+  const int n = tc.n0 + i;
+  const int zoff = tc.batch * p.bias_z_off;
+  sb[i] = (p.scale && n < p.cout) ? __ldg(p.scale + zoff + n) : 1.f;
+  sb[bias_off + i] = (p.bias && n < p.cout) ? __ldg(p.bias + zoff + n) : 0.f;
+}
+
+// ------------------------------------------------------------------ TMA producer
+struct PipeState {
+  int stage;
+  uint32_t phase;
+};
+
+// The loads of k-blocks [kb0, kb1) of one tile pass into the STAGES-deep ring of stages stage_bytes apart from stage0, by
+// lanes 0 and 1 of the producer warp, so that the two descriptor-based copies of a k-block are issued in parallel. Lane 0
+// posts the stage's tx_bytes and loads the A tile (the tile's pixel rectangle shifted to filter tap (r, s)); lane 1 loads
+// B rows n0 .. to b_off and, if b_lo_off != 0, their pre-split low parts (taps + p.b_lo_tap_off) to b_lo_off. bk: K slab
+// width in elements. on_stage(kb) runs once the stage of k-block kb is free.
+template <int STAGES, class F>
+__device__ __forceinline__ void produce_pass(const CUtensorMap* tmA, const CUtensorMap* tmB, uint64_t* full_bar,
+                                             uint64_t* empty_bar, PipeState& ps, uint8_t* stage0, int stage_bytes, int b_off,
+                                             int b_lo_off, int bk, uint32_t tx_bytes, const ConvGemmParams& p,
+                                             const TileCoord& tc, int n0, int kb0, int kb1, int lane, F&& on_stage) {
+  const int k_chunks = p.k_chunks, taps_s = p.taps_s;
+  int tap = kb0 / k_chunks;
+  int kc = kb0 - tap * k_chunks;
+  int r = tap / taps_s;
+  int sx = tap - r * taps_s;
+  const int a_c0 = tc.batch * p.a_c_off, a_n = tc.img + tc.batch * p.a_n_off;
+  const int b_k0 = tc.batch * p.b_k_off, b_n = n0 + tc.batch * p.b_n_off;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&empty_bar[ps.stage], ps.phase ^ 1);
+    on_stage(kb);
+    uint8_t* dst = stage0 + ps.stage * stage_bytes;
+    if (lane == 0) {
+      mbar_arrive_expect_tx(&full_bar[ps.stage], tx_bytes);
+      tma_load_4d(dst, tmA, &full_bar[ps.stage], kc * bk + a_c0, tc.w0 * p.stride_w + sx * p.dil - p.pad_w,
+                  tc.h0 * p.stride_h + r * p.dil - p.pad, a_n);
+    } else {
+      tma_load_3d(dst + b_off, tmB, &full_bar[ps.stage], kc * bk + b_k0, b_n, tap);
+      if (b_lo_off != 0) tma_load_3d(dst + b_lo_off, tmB, &full_bar[ps.stage], kc * bk + b_k0, b_n, tap + p.b_lo_tap_off);
+    }
+    if (++kc == k_chunks) {
+      kc = 0;
+      ++tap;
+      if (++sx == taps_s) {
+        sx = 0;
+        ++r;
+      }
+    }
+    if (++ps.stage == STAGES) {
+      ps.stage = 0;
+      ps.phase ^= 1;
+    }
+  }
+}
 
 // epilogue side of the accumulator ring: this thread's tile row `row`, the 32 columns of the `use`-th chunk that goes through
 // ring slot `slot`; the slot is handed back once the warp has read it (all 32 lanes call this).
@@ -504,51 +646,18 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   griddep_launch_dependents();  // let the next kernel's prologue overlap this kernel
   if (warp == 0) {
     // ===================== TMA producer =====================
-    // lane 0 loads the A (activation) tile and posts the expected byte count, lane 1 the B (weight) tile, so the two
-    // descriptor-based copies of a k-block are issued in parallel; tap / chunk indices advance incrementally
     if (lane < 2) {
-      int stage = 0;
-      uint32_t phase = 0;
+      PipeState ps = {0, 0};
       WorkIter it(p, cta, grid);
       int t;
       int kb0, kb1;
-      const int k_chunks = p.k_chunks, taps_s = p.taps_s;
+      const bool b_lo = SPLIT3 && p.b_lo_tap_off > 0;    // pre-split weights: the low parts come by TMA too
       while (it.next(t, kb0, kb1)) {
-       const TileCoord tc = decode_tile(p, t, BN);
-       for (int pass = 0; pass < (BN > pass_n(BN) ? 2 : 1); ++pass) {
-        int tap = kb0 / k_chunks;
-        int kc = kb0 - tap * k_chunks;
-        int r = tap / taps_s;
-        int sx = tap - r * taps_s;
-        const int a_c0 = tc.batch * p.a_c_off, a_n = tc.img + tc.batch * p.a_n_off;
-        const int b_k0 = tc.batch * p.b_k_off, b_n = tc.n0 + pass * pass_n(BN) + tc.batch * p.b_n_off;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* a_dst = smem + stage * L::kStageBytes;
-          const bool b_lo_ready = SPLIT3 && p.b_lo_tap_off > 0;    // pre-split weights: the low parts come by TMA too
-          if (lane == 0) {
-            mbar_arrive_expect_tx(&full_bar[stage], L::kHalf + (b_lo_ready ? L::kBBytes : 0));   // bytes the TMA loads deliver
-            tma_load_4d(a_dst, &tmA, &full_bar[stage], kc * kBK + a_c0, tc.w0 * p.stride_w + sx * p.dil - p.pad_w,
-                        tc.h0 * p.stride_h + r * p.dil - p.pad, a_n);
-          } else {
-            tma_load_3d(a_dst + L::kABytes, &tmB, &full_bar[stage], kc * kBK + b_k0, b_n, tap);
-            if (b_lo_ready)
-              tma_load_3d(a_dst + L::kABytes + L::kBBytes, &tmB, &full_bar[stage], kc * kBK + b_k0, b_n, tap + p.b_lo_tap_off);
-          }
-          if (++kc == k_chunks) {
-            kc = 0;
-            ++tap;
-            if (++sx == taps_s) {
-              sx = 0;
-              ++r;
-            }
-          }
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-       }
+        const TileCoord tc = decode_tile(p, t, BN);
+        for (int pass = 0; pass < (BN > pass_n(BN) ? 2 : 1); ++pass)
+          produce_pass<STAGES>(&tmA, &tmB, full_bar, empty_bar, ps, smem, L::kStageBytes, L::kABytes,
+                               b_lo ? L::kABytes + L::kBBytes : 0, kBK, L::kHalf + (b_lo ? L::kBBytes : 0), p, tc,
+                               tc.n0 + pass * pass_n(BN), kb0, kb1, lane, [](int) {});
       }
     }
   } else if (warp >= kMmaWarp0) {
@@ -632,20 +741,17 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item, seq0 += BN / 32) {
       const TileCoord tc = decode_tile(p, t, BN);
       const bool complete = (kb0 == 0 && kb1 == KB);
-      const int r0 = q * 32;
-      const int bh0 = r0 / p.tile_w, bw0 = r0 - bh0 * p.tile_w;
-      const int st_w = tc.w0 + bw0, st_h = tc.h0 + bh0;
-      const int res_n = tc.img + tc.batch * p.res_n_off;
+      const StoreBox box = store_box(p, tc, q);
       const int nchunks = min(BN / 32, (p.cout - tc.n0 + 31) / 32);
       const int bsel = tile_item & 1;
       // ---- bias slices: [bsel] holds this tile's (written at the end of the previous tile, or right here for the first)
-      epi_bar_sync8();     // every warp is done with the tile before: its bias buffer may be refilled, this one's is visible
+      epi_bar_sync<256>();     // every warp is done with the tile before: its bias buffer may be refilled, this one's is visible
       if (tile_item == 0) {
         if (epi_tid < BN) {
           const int n = tc.n0 + epi_tid;
           bias_s[epi_tid] = (p.bias && n < p.cout) ? __ldg(p.bias + tc.batch * p.bias_z_off + n) : 0.f;
         }
-        epi_bar_sync8();
+        epi_bar_sync<256>();
       }
       float next_bias = 0.f;
       bool has_next = false;
@@ -669,7 +775,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const int cj = 2 * j + half;
             if (cj < nchunks) {
               mbar_arrive_expect_tx(&rbar[j], 4096);
-              tma_load_4d(stage_buf + j * 4096, &tmRes, &rbar[j], tc.n0 + cj * 32 + tc.batch * p.res_c_off, st_w, st_h, res_n);
+              tma_load_4d(stage_buf + j * 4096, &tmRes, &rbar[j], tc.n0 + cj * 32 + tc.batch * p.res_c_off, box.w, box.h,
+                          box.res_n);
             }
           }
         }
@@ -685,32 +792,15 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       int c_first = cta, c_last = cta;
       if (!complete) {
         // ---- publish this CTA's partial accumulator (my chunks), then find out whether it arrived last
-        float* my_ws = p.part_ws + ((static_cast<long long>(cta) * 2 + (tile_item == 0 ? 0 : 1)) * kBM + row) * BN;
+        float* part = sk_own_part_row(p, cta, tile_item, row, BN);
 #pragma unroll
         for (int j = 0; j < kCPW; ++j) {
-          float acc[32];
-          load_chunk(j, acc);
-#pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            __stcg(reinterpret_cast<float4*>(my_ws + (2 * j + half) * 32 + i), make_float4(acc[i], acc[i + 1], acc[i + 2], acc[i + 3]));
+          uint32_t raw[32];
+          ring_take(ring, ring_full, ring_empty, seq0 + 2 * j + half, row, raw);
+          sk_publish(part, (2 * j + half) * 32, raw);
         }
-        __threadfence();
-        epi_bar_sync8();
-        c_first = unit_owner(U, grid, t * KB);
-        c_last = unit_owner(U, grid, t * KB + KB - 1);
-        if (epi_tid == 0) {
-          const int parts = c_last - c_first + 1;
-          const int old = atomicAdd(&p.counters[t], 1);
-          const int last = (old == parts - 1);
-          if (last) p.counters[t] = 0;   // every part has arrived: leave the counter clean for the next launch
-          *epi_flag = last;
-        }
-        epi_bar_sync8();
-        finalize = (*epi_flag != 0);
-        if (finalize) {
-          __threadfence();
-          issue_residual();
-        }
+        finalize = sk_elect_finisher<256>(p, U, grid, KB, t, epi_tid, epi_flag, c_first, c_last);
+        if (finalize) issue_residual();
       }
       if (finalize) {
         const int out_n = tc.img + tc.batch * p.out_n_off;
@@ -719,22 +809,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const int cj = 2 * j + half;
           if (cj < nchunks) {
             float acc[32];
-            if (complete) {
-              load_chunk(j, acc);
-            } else {
-              // deterministic reduction: parts summed in CTA order (this CTA's own part as published above)
-#pragma unroll
-              for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-              for (int oc = c_first; oc <= c_last; ++oc) {
-                const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
-                const float* ws = p.part_ws + ((static_cast<long long>(oc) * 2 + slot) * kBM + row) * BN + cj * 32;
-#pragma unroll
-                for (int i = 0; i < 32; i += 4) {
-                  const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + i));
-                  acc[i] += v.x; acc[i + 1] += v.y; acc[i + 2] += v.z; acc[i + 3] += v.w;
-                }
-              }
-            }
+            if (complete) load_chunk(j, acc);
+            else sk_reduce(p, U, grid, KB, t, c_first, c_last, row, BN, cj * 32, acc);
             uint8_t* rowp = stage_buf + j * 4096 + lane * 128;
             const float4* biv = reinterpret_cast<const float4*>(bias_s + bsel * BN + cj * 32);
 #pragma unroll
@@ -794,7 +870,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             fence_async_smem();
             __syncwarp();
             if (lane == 0) {
-              tma_store_4d(&tmOut, stage_buf + j * 4096, tc.n0 + cj * 32 + tc.batch * p.out_c_off, st_w, st_h, out_n);
+              tma_store_4d(&tmOut, stage_buf + j * 4096, tc.n0 + cj * 32 + tc.batch * p.out_c_off, box.w, box.h, out_n);
               tma_store_commit();
             }
           } else if (complete) {
@@ -824,54 +900,27 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const bool complete = (kb0 == 0 && kb1 == KB);
       // ---- while the MMAs of this tile run: stage its scale / bias slice in shared memory (the chunk loop then reads
       //      them with broadcast LDS instead of L1-missing global loads) and start the first residual load
-      const int r0 = q * 32;
-      const int bh0 = r0 / p.tile_w, bw0 = r0 - bh0 * p.tile_w;
-      const int st_w = tc.w0 + bw0, st_h = tc.h0 + bh0;
-      const int res_n = tc.img + tc.batch * p.res_n_off;
+      const StoreBox box = store_box(p, tc, q);
       const int nchunks = min(BN / CW, (p.cout - tc.n0 + CW - 1) / CW);
-      epi_bar_sync();   // every warp is done with the previous tile's scale / bias
-      for (int i = epi_tid; i < BN; i += 128) {
-        const int n = tc.n0 + i;
-        const int zoff = tc.batch * p.bias_z_off;
-        sb_s[i] = (p.scale && n < p.cout) ? __ldg(p.scale + zoff + n) : 1.f;
-        sb_s[L::kSbCols + i] = (p.bias && n < p.cout) ? __ldg(p.bias + zoff + n) : 0.f;
-      }
+      epi_bar_sync<128>();   // every warp is done with the previous tile's scale / bias
+      for (int i = epi_tid; i < BN; i += 128) stage_scale_bias(sb_s, L::kSbCols, p, tc, i);
       if (complete && p.has_residual && lane == 0 && nchunks > 0) {
         mbar_arrive_expect_tx(&rbar[0], 4096);
-        tma_load_4d(epi_res, &tmRes, &rbar[0], tc.n0 + tc.batch * p.res_c_off, st_w, st_h, res_n);
+        tma_load_4d(epi_res, &tmRes, &rbar[0], tc.n0 + tc.batch * p.res_c_off, box.w, box.h, box.res_n);
       }
-      epi_bar_sync();
+      epi_bar_sync<128>();
       bool finalize = complete;
       int c_first = cta, c_last = cta;
       if (!complete) {
         // ---- publish this CTA's partial accumulator, then find out whether it arrived last
-        float* my_ws = p.part_ws + ((static_cast<long long>(cta) * 2 + (tile_item == 0 ? 0 : 1)) * kBM + row) * BN;
-        auto publish = [&](const int c) {
-          uint32_t acc[32];
-          ring_take(ring, ring_full, ring_empty, seq0 + c, row, acc);
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 v = make_float4(__uint_as_float(acc[j]), __uint_as_float(acc[j + 1]),
-                                   __uint_as_float(acc[j + 2]), __uint_as_float(acc[j + 3]));
-            __stcg(reinterpret_cast<float4*>(my_ws + c * 32 + j), v);
-          }
-        };
+        float* part = sk_own_part_row(p, cta, tile_item, row, BN);
 #pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) publish(c);
-        __threadfence();
-        epi_bar_sync();
-        c_first = unit_owner(U, grid, t * KB);
-        c_last = unit_owner(U, grid, t * KB + KB - 1);
-        if (epi_tid == 0) {
-          const int parts = c_last - c_first + 1;
-          const int old = atomicAdd(&p.counters[t], 1);
-          const int last = (old == parts - 1);
-          if (last) p.counters[t] = 0;   // every part has arrived: leave the counter clean for the next launch
-          *epi_flag = last;
+        for (int c = 0; c < BN / 32; ++c) {
+          uint32_t raw[32];
+          ring_take(ring, ring_full, ring_empty, seq0 + c, row, raw);
+          sk_publish(part, c * 32, raw);
         }
-        epi_bar_sync();
-        finalize = (*epi_flag != 0);
-        if (finalize) __threadfence();
+        finalize = sk_elect_finisher<128>(p, U, grid, KB, t, epi_tid, epi_flag, c_first, c_last);
       }
       if (finalize) {
         // Output pixels of this warp: tile rows [32q, 32q+32) = a box_h x box_w rectangle. Results go
@@ -882,7 +931,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const uint32_t sw = static_cast<uint32_t>(lane & 7);
         if (!complete && p.has_residual && lane == 0 && nchunks > 0) {   // (whole tiles started this load earlier)
           mbar_arrive_expect_tx(&rbar[0], 4096);
-          tma_load_4d(epi_res, &tmRes, &rbar[0], tc.n0 + tc.batch * p.res_c_off, st_w, st_h, res_n);
+          tma_load_4d(epi_res, &tmRes, &rbar[0], tc.n0 + tc.batch * p.res_c_off, box.w, box.h, box.res_n);
         }
         auto finish_chunk = [&](const int c) {
           const int nb = tc.n0 + c * CW;
@@ -891,8 +940,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const int rb = c & 1;
             if (c + 1 < nchunks && lane == 0) {   // prefetch the next residual chunk into the other buffer
               mbar_arrive_expect_tx(&rbar[rb ^ 1], 4096);
-              tma_load_4d(epi_res + (rb ^ 1) * 4096, &tmRes, &rbar[rb ^ 1], nb + CW + tc.batch * p.res_c_off, st_w, st_h,
-                          res_n);
+              tma_load_4d(epi_res + (rb ^ 1) * 4096, &tmRes, &rbar[rb ^ 1], nb + CW + tc.batch * p.res_c_off, box.w, box.h,
+                          box.res_n);
             }
             mbar_wait(&rbar[rb], (rphase >> rb) & 1u);
             rphase ^= (1u << rb);
@@ -913,18 +962,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         #pragma unroll
               for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(raw[j]);
             } else {
-              // deterministic reduction: parts summed in CTA order (this CTA's own part as published above)
-        #pragma unroll
-              for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-              for (int oc = c_first; oc <= c_last; ++oc) {
-                const int slot = (cta_first_unit(U, grid, oc) >= t * KB) ? 0 : 1;
-                const float* ws = p.part_ws + ((static_cast<long long>(oc) * 2 + slot) * kBM + row) * BN + col0;
-        #pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                  const float4 v = __ldcg(reinterpret_cast<const float4*>(ws + j));
-                  acc[j] += v.x; acc[j + 1] += v.y; acc[j + 2] += v.z; acc[j + 3] += v.w;
-                }
-              }
+              sk_reduce(p, U, grid, KB, t, c_first, c_last, row, BN, col0, acc);
             }
             if (has_sb) {
               const float4* scv = reinterpret_cast<const float4*>(sb_s + col0);
@@ -980,7 +1018,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           fence_async_smem();
           __syncwarp();
           if (lane == 0) {
-            tma_store_4d(&tmOut, epi_out + (c & 1) * 4096, nb + tc.batch * p.out_c_off, st_w, st_h, out_n);
+            tma_store_4d(&tmOut, epi_out + (c & 1) * 4096, nb + tc.batch * p.out_c_off, box.w, box.h, out_n);
             tma_store_commit();
           }
         };
@@ -1024,32 +1062,53 @@ static int launch_cfg(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUte
   return MEGA_OK;
 }
 
-// the instantiation of a grouped launch's group width (block_n 64)
-template <int STAGES, int MODE, bool OUT16>
-static int launch_grouped(int gw, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
-                          const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid, cudaStream_t stream, int pdl) {
+// The kernel instantiation of one launch of operand mode MODE: block_n, out16 (fp16 output for kModeF16, which needs
+// block_n % 64 == 0; split-fp16 output for kModeF16x3) and the group width gw (0: dense; 8 / 16 / 32: block_n 64).
+// Each mode is instantiated in one translation unit (conv_gemm.cu: tf32 and 3xTF32, conv_gemm_f16.cu, conv_gemm_f16x3.cu),
+// so that nvcc builds them in parallel.
+template <int MODE>
+int launch_mode(int block_n, bool out16, int gw, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
+                const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid, cudaStream_t stream, int pdl) {
+  auto launch = [&](auto bn, auto gw_c) -> int {
+    constexpr int BN = decltype(bn)::value, GW = decltype(gw_c)::value, ST = conv_gemm_stages(MODE, BN);
+    if constexpr (MODE == kModeF16x3 || (MODE == kModeF16 && BN % 64 == 0)) {
+      if (out16) return launch_cfg<BN, ST, MODE, true, GW>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    } else if (out16) {
+      mega_set_error("conv_gemm: fp16 output needs fp16 operands and block_n %% 64 == 0 (got precision %d, block_n %d)",
+                     MODE, BN);
+      return MEGA_ERR_ARG;
+    }
+    return launch_cfg<BN, ST, MODE, false, GW>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+  };
   switch (gw) {
-    case 8: return launch_cfg<64, STAGES, MODE, OUT16, 8>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    case 16: return launch_cfg<64, STAGES, MODE, OUT16, 16>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
-    default: return launch_cfg<64, STAGES, MODE, OUT16, 32>(tmA, tmB, tmOut, tmRes, p, grid, stream, pdl);
+    case 8: return launch(IntC<64>(), IntC<8>());
+    case 16: return launch(IntC<64>(), IntC<16>());
+    case 32: return launch(IntC<64>(), IntC<32>());
   }
+  switch (block_n) {
+    case 64: return launch(IntC<64>(), IntC<0>());
+    case 128: return launch(IntC<128>(), IntC<0>());
+  }
+  if constexpr (MODE == kModeTf32 || MODE == kModeF16) {   // the strict modes run block_n 64 and 128 only
+    switch (block_n) {
+      case 32: return launch(IntC<32>(), IntC<0>());
+      case 96: return launch(IntC<96>(), IntC<0>());
+      case 160: return launch(IntC<160>(), IntC<0>());
+      case 192: return launch(IntC<192>(), IntC<0>());
+      case 256: return launch(IntC<256>(), IntC<0>());
+    }
+  }
+  mega_set_error("conv_gemm: unsupported block_n %d for precision %d", block_n, MODE);
+  return MEGA_ERR_ARG;
 }
 
-// fp16-operand instantiations live in their own translation unit (conv_gemm_f16.cu)
-int launch_conv_gemm_f16(int block_n, int out_f16, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                         const CUtensorMap& tmOut, const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid,
-                         cudaStream_t stream, int pdl);
-
-// grouped launches (group width gw = 8 / 16 / 32, block_n 64) of the fp16 / split-fp16 modes
-int launch_conv_gemm_f16_grouped(int gw, int out_f16, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut,
-                                 const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid, cudaStream_t stream, int pdl);
-int launch_conv_gemm_f16x3_grouped(int gw, int out_split, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                                   const CUtensorMap& tmOut, const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid,
-                                   cudaStream_t stream, int pdl);
-
-// split-fp16 ("3xFP16") instantiations: conv_gemm_f16x3.cu
-int launch_conv_gemm_f16x3(int block_n, int out_split, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                           const CUtensorMap& tmOut, const CUtensorMap& tmRes, const ConvGemmParams& p, dim3 grid,
-                           cudaStream_t stream, int pdl);
+// declarator of launch_mode<M> for its explicit instantiations
+#define MEGA_LAUNCH_MODE(M)                                                                                                \
+  int launch_mode<M>(int, bool, int, const CUtensorMap&, const CUtensorMap&, const CUtensorMap&, const CUtensorMap&,     \
+                     const ConvGemmParams&, dim3, cudaStream_t, int)
+extern template MEGA_LAUNCH_MODE(kModeTf32);
+extern template MEGA_LAUNCH_MODE(kModeSplit3);
+extern template MEGA_LAUNCH_MODE(kModeF16);
+extern template MEGA_LAUNCH_MODE(kModeF16x3);
 
 }  // namespace mega
