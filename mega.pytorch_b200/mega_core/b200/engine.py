@@ -44,9 +44,9 @@ class EngineConfig:
     key_frame_location = 12
     memory_size = 25
     global_size = 10
-    global_res_stage = 1
-    stage = 3
-    advanced_stage = 0           # RDN: MODEL.VID.ROI_BOX_HEAD.ATTENTION.ADVANCED_STAGE
+    global_res_stage = 1         # MEGA: MODEL.VID.MEGA.GLOBAL.RES_STAGE, 0 or 1
+    stage = 3                    # MODEL.VID.ROI_BOX_HEAD.ATTENTION.STAGE: 3 (MEGA) or 2 (RDN)
+    advanced_stage = 0           # RDN: MODEL.VID.ROI_BOX_HEAD.ATTENTION.ADVANCED_STAGE, 0 or 1
     groups = 16
     pooler_resolution = 7
     pooler_scale = 1.0 / 16
@@ -392,6 +392,10 @@ class HeadCommon:
         assert self.base_anchors.shape[0] == a
         self.res5 = ResNetStages(sd, FE + "head.", (4,), dev, dilation=cfg.res5_dilation,
                                  first_stride_of=lambda li: 1, dtype=act)
+        self.reduce = (FE + "conv.weight") in sd          # REDUCE_CHANNEL: 1x1 conv 2048 -> 256 + ReLU after res5
+        if self.reduce:
+            self.red_w = pack_conv(sd[FE + "conv.weight"], dev, act)
+            self.red_b = sd[FE + "conv.bias"].float().contiguous().to(dev)
         pw = torch.cat([sd["roi_heads.box.predictor.cls_score.weight"].float(),
                         sd["roi_heads.box.predictor.bbox_pred.weight"].float()], 0)
         self.num_classes = sd["roi_heads.box.predictor.cls_score.weight"].shape[0]
@@ -412,6 +416,35 @@ class HeadCommon:
             t = torch.zeros(*shape, device=self.dev, dtype=dtype)
             self._bufs[key] = t
         return t
+
+    def res5_reduced(self, feats, ch=None, max_ctas=0):
+        """res5 (+ the channel-reduction conv and its ReLU, extractors :274-283 / :474-483) on the backbone map, as layers
+        of the caller's open chain `ch`; ch.interleave: the two halves of the batch run as the chain's two lanes, each
+        lane's reduction after its own res5 layers"""
+        if ch is not None and ch.interleave:
+            r5 = self._buf("res5_out", self.res5.out_shape(feats.shape), self.act)
+            if not self.reduce:
+                return self.res5.forward_lanes(feats, ch, r5, max_ctas=max_ctas)
+            out = self._reduce_buf(r5.shape)
+            h = feats.shape[0] // 2
+            self.res5.forward_lanes(feats, ch, r5, max_ctas=max_ctas,
+                                    tail=lambda y, lane: self._reduce(y, out[lane * h:(lane + 1) * h], max_ctas))
+            return out
+        x = self.res5.forward(feats, max_ctas=max_ctas)
+        if self.reduce:
+            x = self._reduce(x, self._reduce_buf(x.shape), max_ctas)
+        return x
+
+    def _reduce_buf(self, shape):
+        n, h, w, _ = shape
+        t = self._buf("reduce", (n, h, w, self.red_w.shape[1]), self.act)
+        if getattr(self, "split16", False):
+            ops.mark_split16(t)          # strict mode: split-fp16 map, read by the split-fp16 ROIAlign
+        return t
+
+    def _reduce(self, x, out, max_ctas=0):
+        ops.conv_gemm(x, self.red_w, out, bias=self.red_b, relu=True, max_ctas=max_ctas)
+        return out
 
     def rpn_head(self, feats, lane=None, n_total=None):
         """RPNHead.forward (rpn/rpn.py:99-106): 3x3 conv + ReLU, then objectness and box deltas as one 1x1 GEMM.
@@ -524,10 +557,6 @@ class MlpHeadMixin:
     def _init_mlp_head(self, sd):
         dev, act = self.dev, self.act
         res = self.cfg.pooler_resolution
-        self.reduce = (FE + "conv.weight") in sd
-        if self.reduce:
-            self.red_w = pack_conv(sd[FE + "conv.weight"], dev, act)
-            self.red_b = sd[FE + "conv.bias"].float().contiguous().to(dev)
         w6 = sd[FE + "fc6.weight"].float()
         ch = w6.shape[1] // (res * res)
         self.ch = ch
@@ -544,12 +573,7 @@ class MlpHeadMixin:
         KP = c.post_nms_top_n
         boxes, _, cnt = self.rpn(feats, im_w, im_h, KP)
         with ops.chain(self._chains, ("res5", tuple(feats.shape)), self.dev, enabled=self.chained):
-            x = self.res5.forward(feats)
-            if self.reduce:
-                n, h, w, _ = x.shape
-                xr = self._buf("reduce", (n, h, w, self.red_w.shape[1]), self.act)
-                ops.conv_gemm(x, self.red_w, xr, bias=self.red_b, relu=True)
-                x = xr
+            x = self.res5_reduced(feats)
         res = c.pooler_resolution
         pooled = self._buf("pooled", (KP, res * res * self.ch), self.act)
         ops.roi_align_nhwc(x, boxes[0], None, c.pooler_scale, res, res, c.sampling_ratio, pooled)
@@ -589,7 +613,7 @@ class WindowedEngine(HeadCommon):
         return t
 
     def ref_branch(self, imgs, kinds, im_w, im_h):
-        """backbone -> RPN(300) -> res5 -> ROIAlign -> l_fcs[0]+ReLU for a batch of frames.
+        """backbone -> RPN(300) -> res5 (+ reduction) -> ROIAlign -> l_fcs[0]+ReLU for a batch of frames.
         kinds[i] == "L": local frame (keeps 300 rows); "G": global frame (keeps its first 75).
         returns (x rows [sum r_i, 1024], boxes [n,300,4], cnt [n], spans)"""
         c = self.cfg
@@ -618,11 +642,7 @@ class WindowedEngine(HeadCommon):
         dual = self.chained and ops.DUAL_CHAIN[0] and n >= ops.DUAL_MIN_IMAGES and n % 2 == 0
         with ops.chain(self._chains, ("res5", tuple(feats.shape), dual), self.dev, enabled=self.chained, max_ctas=mc,
                        interleave=dual) as ch:
-            if dual and ch.interleave:
-                r5 = self.res5.forward_lanes(feats, ch, self._buf("res5_out", self.res5.out_shape(feats.shape), self.act),
-                                             max_ctas=mc)
-            else:
-                r5 = self.res5.forward(feats, max_ctas=mc)
+            r5 = self.res5_reduced(feats, ch if dual else None, max_ctas=mc)
         main.wait_stream(self._side)
         src, bidx, spans = self._roi_table(kinds)
         rows = src.numel()
@@ -647,6 +667,8 @@ class WindowedEngine(HeadCommon):
             self.res5.use_split16()
             self.rpn_w, self.rpn_hw = ops.pack_weights_split16(self.rpn_w), ops.pack_weights_split16(self.rpn_hw)
             self.fc0_w = ops.pack_weights_split16(self.fc0_w)
+            if self.reduce:
+                self.red_w = ops.pack_weights_split16(self.red_w)
         else:
             for stages in (self.backbone.stages, self.res5):
                 for blocks in stages.stages:
@@ -656,6 +678,8 @@ class WindowedEngine(HeadCommon):
                                 setattr(blk, name, ops.presplit(getattr(blk, name)))
             self.rpn_w, self.rpn_hw = ops.presplit(self.rpn_w), ops.presplit(self.rpn_hw)
             self.fc0_w = ops.presplit(self.fc0_w)
+            if self.reduce:
+                self.red_w = ops.presplit(self.red_w)
         self.backbone.stem_wr = ops.presplit(self.backbone.stem_wr)
         atts = list(getattr(self, "att_l", [])) + list(getattr(self, "att_g", [])) + list(getattr(self, "att", []))
         self.split16_att = self.split16 and bool(ops.SPLIT16_ATT[0])
@@ -702,14 +726,14 @@ class WindowedEngine(HeadCommon):
 
     @_with_precision
     def roi_features(self, feats_nchw, boxes, batch_idx=None):
-        """feature_extractor(x, proposals, pre_calculate=True) (extractors :885-896): res5 on the map, ROIAlign of the
-        given boxes [K,4] (image index per box in batch_idx, int32), fcs[0] + ReLU -> [K, 1024] fp32"""
+        """feature_extractor(x, proposals, pre_calculate=True) (extractors :885-896): res5 (+ reduction) on the map,
+        ROIAlign of the given boxes [K,4] (image index per box in batch_idx, int32), fcs[0] + ReLU -> [K, 1024] fp32"""
         c = self.cfg
         k = boxes.shape[0]
         assert k <= self.pooled.shape[0], "at most %d rois per call" % self.pooled.shape[0]
         feats = self.to_nhwc(feats_nchw)
         with ops.chain(self._chains, ("res5x", tuple(feats.shape)), self.dev, enabled=self.chained):
-            r5 = self.res5.forward(feats)
+            r5 = self.res5_reduced(feats)
         rb = self.roi_boxes[:k]
         rb.copy_(boxes)
         pooled = self.pooled[:k]
@@ -792,7 +816,10 @@ class WindowedEngine(HeadCommon):
 
 class MegaEngine(WindowedEngine, WavefrontMixin):
     """GeneralizedRCNNMEGA._forward_test + MEGAFeatureExtractor test path
-    (detector/generalized_rcnn_mega.py:137-225; extractors :657-699, :754-774, :806-829, :885-933)."""
+    (detector/generalized_rcnn_mega.py:137-225; extractors :657-699, :754-774, :806-829, :885-933).
+    Served layouts: ATTENTION.STAGE = 3 local stages; MEGA.GLOBAL.RES_STAGE = 1 (configs/MEGA/vid_R_101_C4_MEGA_1x.yaml:
+    a second global stage G1 after the local ones) or 0 (vid_R_50_C4_MEGA_1x.yaml: the key rows of stage 2 go to the
+    predictor); with or without REDUCE_CHANNEL."""
     MAX_FRAMES_PER_STEP = 8      # key frames whose per-frame branch stepn_batched may run as one batch
 
     def __init__(self, sd, cfg=None, device="cuda"):
@@ -802,7 +829,7 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
         c = cfg
         self.R, self.A, self.L, self.KP = c.ref_post_nms_top_n, c.advanced_num, c.all_frame_interval, c.post_nms_top_n
         self.GF, self.MEMF = c.global_size, c.memory_size
-        assert c.stage == 3 and c.global_res_stage == 1, "engine is laid out for STAGE=3, GLOBAL.RES_STAGE=1"
+        assert c.stage == 3 and c.global_res_stage in (0, 1), "engine is laid out for STAGE=3, GLOBAL.RES_STAGE 0 or 1"
         R, A, L, KP, GF = self.R, self.A, self.L, self.KP, self.GF
         res = c.pooler_resolution
         # l_fcs[0]: reference column index c*49 + bin -> bin*2048 + c (ROIAlign output is bin-major here)
@@ -815,7 +842,7 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
         self.fc_w = [None] + [sd[FE + "l_fcs.%d.weight" % i].float().contiguous().to(dev).to(act) for i in (1, 2)]
         self.fc_b = [None] + [sd[FE + "l_fcs.%d.bias" % i].float().contiguous().to(dev) for i in (1, 2)]
         self.att_l = [_Att(sd, FE + "l_", i, dev, True, act) for i in range(3)]
-        self.att_g = [_Att(sd, FE + "g_", i, dev, False, act) for i in range(2)]
+        self.att_g = [_Att(sd, FE + "g_", i, dev, False, act) for i in range(c.global_res_stage + 1)]
         self.feat_dim = 1024
         D = self.feat_dim
         z = lambda *s, dtype=torch.float32: torch.zeros(*s, device=dev, dtype=dtype)
@@ -832,7 +859,8 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
         self.Qin0, self.Bq0 = za(self.nq, D), z(self.nq, 4)
         self.Y1E, self.Y2M = za(self.nq + self.mem_cap12, D), za(self.nq + self.mem_cap12, D)
         self.B1, self.B2 = z(self.nl12 + self.mem_cap12, 4), z(self.nl12 + self.mem_cap12, 4)
-        self.X1, self.X2, self.X3, self.X4 = za(self.nq, D), za(self.nq, D), za(KP, D), za(KP, D)
+        self.X1, self.X2, self.X3 = za(self.nq, D), za(self.nq, D), za(KP, D)
+        self.X4 = za(KP, D) if c.global_res_stage else None
         self.cur_cnt = z(1, 1, dtype=torch.int32)
         self.payload_in = z(KP * self.fw + KP * 4 + 4 + R * self.fw)   # 32-bit words: x300 | boxes | count | x75
         self.payload_all = None
@@ -1209,13 +1237,26 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
                         tail=lambda: ops.linear(self.X2, self.fc_w[2], self.Y2M[:nq], bias=self.fc_b[2], relu=True))
         self._push_mem12(self.Y1E, self.B1)
         # stage 2 (key rows only)
-        self._attention(self.att_l[2], self.Y2M[:KP], KP, self.Y2M[KP:], nl12 + self.mem_cap12, self.ld_12, self.X3,
-                        boxes_q=self.Bq0[:KP], boxes_k=self.B2, m_valid=mv[2:3])
+        self._stage2(mv)
         self._push_mem12(self.Y2M, self.B2)
-        # G1: update_lm(x, 1) (extractors :930-931)
-        self._attention(self.att_g[1], self.X3, KP, self.glob_x, self.GF * R, self.ld_g, self.X4,
-                        tail=lambda: self.predict_gemm(self.X4))       # the predictor rides in the last P.V' chain
-        return self.predict_and_postprocess(self.X4, self.Bq0[:KP], kcnt, im_w, im_h, gemm_done=True)
+        x = self._global_res()
+        return self.predict_and_postprocess(x, self.Bq0[:KP], kcnt, im_w, im_h, gemm_done=True)
+
+    def _stage2(self, mv):
+        """local stage 2 on the key rows -> X3; without a global stage after it (GLOBAL.RES_STAGE = 0) X3 is the predictor's
+        input and the predictor GEMM rides in this stage's P.V' chain"""
+        tail = (lambda: self.predict_gemm(self.X3)) if self.cfg.global_res_stage == 0 else None
+        self._attention(self.att_l[2], self.Y2M[:self.KP], self.KP, self.Y2M[self.KP:], self.nl12 + self.mem_cap12,
+                        self.ld_12, self.X3, boxes_q=self.Bq0[:self.KP], boxes_k=self.B2, m_valid=mv[2:3], tail=tail)
+
+    def _global_res(self):
+        """G1, update_lm(x, 1) (extractors :930-931), when GLOBAL.RES_STAGE = 1, with the predictor GEMM in its P.V' chain;
+        returns the predictor's input rows (the predictor has run)"""
+        if self.cfg.global_res_stage == 0:
+            return self.X3
+        self._attention(self.att_g[1], self.X3, self.KP, self.glob_x, self.GF * self.R, self.ld_g, self.X4,
+                        tail=lambda: self.predict_gemm(self.X4))
+        return self.X4
 
     def _assemble_window(self):
         """window assembly (replaces the torch.cat of the deques, generalized_rcnn_mega.py:213-216) -> (key count, mvalid)"""
@@ -1284,20 +1325,19 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
         self._push_mem12(self.Y1E, self.B1)
         if owner:
             # stage 2 and G1 have key-row queries only
-            self._attention(self.att_l[2], self.Y2M[:KP], KP, self.Y2M[KP:], m12, self.ld_12, self.X3,
-                            boxes_q=Bq0[:KP], boxes_k=self.B2, m_valid=mv[2:3])
+            self._stage2(mv)
         self._push_mem12(self.Y2M, self.B2)
         if not owner:
             return None
-        self._attention(self.att_g[1], self.X3, KP, self.glob_x, self.GF * R, self.ld_g, self.X4,
-                        tail=lambda: self.predict_gemm(self.X4))
-        return self.predict_and_postprocess(self.X4, Bq0[:KP], kcnt, im_w, im_h, gemm_done=True)
+        x = self._global_res()
+        return self.predict_and_postprocess(x, Bq0[:KP], kcnt, im_w, im_h, gemm_done=True)
 
 
 class RdnEngine(WindowedEngine):
     """GeneralizedRCNNRDN._forward_test + RDNFeatureExtractor test path (detector/generalized_rcnn_rdn.py:108-190;
-    roi_box_feature_extractors.py:400-454 with the base attention module :178-238), ATTENTION.STAGE = 2,
-    ADVANCED_STAGE = 1 (configs/RDN/vid_R_101_C4_RDN_1x.yaml), window of 37 frames with the key frame at 18.
+    roi_box_feature_extractors.py:400-454 with the base attention module :178-238), ATTENTION.STAGE = 2 base stages and
+    ADVANCED_STAGE = 1 (configs/RDN/vid_R_101_C4_RDN_1x.yaml) or 0 (the RDN-base configs: the key rows go to the
+    predictor after base stage 1), with or without REDUCE_CHANNEL; window of 37 frames with the key frame at 18.
 
     Same restructuring as MegaEngine: every frame goes once through backbone -> RPN(300) -> res5 -> ROIAlign ->
     fcs[0] when it ENTERS the window (its 75 reference proposals are the prefix of its 300 key proposals; the
@@ -1309,7 +1349,8 @@ class RdnEngine(WindowedEngine):
         dev = torch.device(device)
         super().__init__(sd, cfg, dev)
         c = cfg
-        assert c.stage == 2 and c.advanced_stage == 1, "engine is laid out for ATTENTION.STAGE=2, ADVANCED_STAGE=1"
+        assert c.stage == 2 and c.advanced_stage in (0, 1), "engine is laid out for ATTENTION.STAGE=2, ADVANCED_STAGE 0 or 1"
+        self.adv = adv = c.advanced_stage
         self.R, self.A, self.L, self.KP = c.ref_post_nms_top_n, c.advanced_num, c.all_frame_interval, c.post_nms_top_n
         R, A, L, KP = self.R, self.A, self.L, self.KP
         res, act = c.pooler_resolution, self.act
@@ -1318,26 +1359,30 @@ class RdnEngine(WindowedEngine):
         self.fc0_w = self.pack_fc0(w0.reshape(w0.shape[0], ch, res * res).permute(0, 2, 1).reshape(w0.shape[0], -1)
                                    .to(act)).to(dev)
         self.fc0_b = sd[FE + "fcs.0.bias"].float().contiguous().to(dev)
-        self.fc_w = [None] + [sd[FE + "fcs.%d.weight" % i].float().contiguous().to(dev).to(act) for i in (1, 2)]
-        self.fc_b = [None] + [sd[FE + "fcs.%d.bias" % i].float().contiguous().to(dev) for i in (1, 2)]
-        self.att = [_Att(sd, FE, i, dev, True, act) for i in range(4)]
+        fcs = (1, 2)[:1 + adv]
+        self.fc_w = [None] + [sd[FE + "fcs.%d.weight" % i].float().contiguous().to(dev).to(act) for i in fcs]
+        self.fc_b = [None] + [sd[FE + "fcs.%d.bias" % i].float().contiguous().to(dev) for i in fcs]
+        self.att = [_Att(sd, FE, i, dev, True, act) for i in range(4 if adv else 2)]
         self.feat_dim = D = 1024
         z = lambda *s, dtype=torch.float32: torch.zeros(*s, device=dev, dtype=dtype)
         za = lambda *s: torch.zeros(*s, device=dev, dtype=act)
         self.win_x, self.win_boxes, self.win_cnt = za(L * KP, D), z(L * KP, 4), z(L, 1, dtype=torch.int32)
         self.nref, self.nadv = L * R, L * A                     # 2775 reference rows, 555 distilled rows
         self.E, self.B = za(KP + self.nref, D), z(KP + self.nref, 4)       # [key 300 | refs 2775]
-        self.Xadv, self.Badv = za(self.nadv, D), z(self.nadv, 4)
-        self.X1, self.Y1, self.X2, self.X3 = za(KP, D), za(KP, D), za(KP, D), za(KP, D)
-        self.Xa, self.Ya = za(self.nadv, D), za(self.nadv, D)
-        self.cur_cnt = z(1, 1, dtype=torch.int32)
+        self.X1, self.Y1, self.X2 = za(KP, D), za(KP, D), za(KP, D)
         self.ld_ref, self.ld_adv = _round_up(self.nref, 32), _round_up(self.nadv, 32)
-        self._alloc_attention([(max(KP, self.nadv), self.ld_ref), (KP, self.ld_adv)], self.nref)
+        if adv:
+            self.Xadv, self.Badv = za(self.nadv, D), z(self.nadv, 4)
+            self.X3, self.Xa, self.Ya = za(KP, D), za(self.nadv, D), za(self.nadv, D)
+            self._alloc_attention([(max(KP, self.nadv), self.ld_ref), (KP, self.ld_adv)], self.nref)
+        else:
+            self._alloc_attention([(KP, self.ld_ref)], self.nref)
+        self.cur_cnt = z(1, 1, dtype=torch.int32)
         self.pooled = za(2 * KP, res * res * ch)                # the first frame of a video runs 2 frames per batch
         self.fc0_out = za(2 * KP, D)
         self.roi_boxes, self.roi_batch = z(2 * KP, 4), z(2 * KP, dtype=torch.int32)
         o, off = {}, 0
-        for name, n in (("idx_e", KP + self.nref), ("idx_adv", self.nadv), ("dst_local", KP), ("slot_new", 4),
+        for name, n in (("idx_e", KP + self.nref), ("idx_adv", self.nadv * adv), ("dst_local", KP), ("slot_new", 4),
                         ("slot_key", 4)):
             o[name] = (off, n)
             off += _round_up(n, 4)
@@ -1379,7 +1424,8 @@ class RdnEngine(WindowedEngine):
         e[:KP] = kslot * KP + np.arange(KP)
         e[KP:] = (sl[:, None] * KP + np.arange(R)[None, :]).reshape(-1)
         th("idx_e").copy_(torch.from_numpy(e))
-        th("idx_adv").copy_(torch.from_numpy((sl[:, None] * KP + np.arange(A)[None, :]).reshape(-1).astype(np.int32)))
+        if self.adv:
+            th("idx_adv").copy_(torch.from_numpy((sl[:, None] * KP + np.arange(A)[None, :]).reshape(-1).astype(np.int32)))
         if slot_new is not None:
             th("dst_local").copy_(torch.arange(slot_new * KP, (slot_new + 1) * KP, dtype=torch.int32))
             th("slot_new")[0] = slot_new
@@ -1436,8 +1482,9 @@ class RdnEngine(WindowedEngine):
         t = self._tab
         ops.gather_rows(self.win_x, t("idx_e"), self.E, KP + nref)
         ops.gather_rows(self.win_boxes, t("idx_e"), self.B, KP + nref)
-        ops.gather_rows(self.win_x, t("idx_adv"), self.Xadv, nadv)
-        ops.gather_rows(self.win_boxes, t("idx_adv"), self.Badv, nadv)
+        if self.adv:
+            ops.gather_rows(self.win_x, t("idx_adv"), self.Xadv, nadv)
+            ops.gather_rows(self.win_boxes, t("idx_adv"), self.Badv, nadv)
         ops.gather_rows(self.win_cnt.view(torch.float32), t("slot_key")[:1], self.cur_cnt.view(torch.float32), 1,
                         row_len=1)
         kcnt = self.cur_cnt.view(-1)[:1]
@@ -1449,13 +1496,15 @@ class RdnEngine(WindowedEngine):
         ops.linear(self.X1, self.fc_w[1], self.Y1, bias=self.fc_b[1], relu=True)
         self._attention(self.att[1], self.Y1, KP, refs, nref, self.ld_ref, self.X2, boxes_q=bk, boxes_k=bref,
                         n_valid=kcnt, n_valid_off=KP)
+        self.last_props = bk
+        if not self.adv:          # RDN-base: the output of base stage 1 is the predictor's input
+            return self.predict_and_postprocess(self.X2, bk, kcnt, im_w, im_h)
         # advanced stage (:438-452): the first 15 rows of every frame attend to all reference rows ...
         self._attention(self.att[2], self.Xadv, nadv, refs, nref, self.ld_ref, self.Xa, boxes_q=self.Badv, boxes_k=bref)
         ops.linear(self.Xa, self.fc_w[2], self.Ya, bias=self.fc_b[2], relu=True)
         # ... and the key rows attend to those 555 distilled rows
         self._attention(self.att[3], self.X2, KP, self.Ya, nadv, self.ld_adv, self.X3, boxes_q=bk, boxes_k=self.Badv,
                         n_valid=kcnt, n_valid_off=KP)
-        self.last_props = bk
         return self.predict_and_postprocess(self.X3, bk, kcnt, im_w, im_h)
 
 

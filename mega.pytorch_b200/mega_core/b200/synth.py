@@ -73,11 +73,18 @@ def _linear(sd, p, nout, nin, gen, std=None, gain=1.0):
     sd[p + "bias"] = torch.randn(nout, generator=gen) * 0.01
 
 
-def make_state_dict(arch="mega_r101", seed=0, num_classes=31):
+def make_state_dict(arch="mega_r101", seed=0, num_classes=31, reduce_channel=False, global_res_stage=1, advanced_stage=1):
     """state_dict with the reference's key names/shapes for
     arch in {"mega_r101", "mega_r50", "rdn_r101", "fgfa_r101", "dff_r101", "base_r50", "base_r101", "mega_x101", "base_x101"}
     (+ "_tiny" suffix: 1 block per stage, for fast CPU tests). x101: ResNeXt-101 32x8d (NUM_GROUPS 32, WIDTH_PER_GROUP 8:
-    bottleneck widths 256 .. 2048, grouped conv2)."""
+    bottleneck widths 256 .. 2048, grouped conv2).
+    MEGA / RDN options of the shipped configs (the defaults give configs/{MEGA,RDN}/vid_R_101_C4_*_1x.yaml):
+      reduce_channel   MODEL.VID.ROI_BOX_HEAD.REDUCE_CHANNEL: the 1x1 conv 2048 -> 256 after res5, l_fcs.0 / fcs.0 read
+                       256 * 49 inputs (configs/MEGA/vid_R_50_C4_MEGA_1x.yaml, configs/RDN/vid_R_50_C4_RDN_base_1x.yaml)
+      global_res_stage MODEL.VID.MEGA.GLOBAL.RES_STAGE: g_* holds global_res_stage + 1 attention modules
+      advanced_stage   MODEL.VID.ROI_BOX_HEAD.ATTENTION.ADVANCED_STAGE of RDN: 0 drops fcs.2 and attention modules 2, 3
+                       (the RDN-base configs)
+    The tensors of the defaults do not depend on these options' existence; the reduction conv is drawn last."""
     gen = torch.Generator().manual_seed(seed)
     tiny = arch.endswith("_tiny")
     base = arch.replace("_tiny", "")
@@ -148,10 +155,10 @@ def make_state_dict(arch="mega_r101", seed=0, num_classes=31):
     elif method == "rdn":
         # RDNFeatureExtractor with ATTENTION.STAGE = 2, ADVANCED_STAGE = 1 (configs/RDN/vid_R_101_C4_RDN_1x.yaml):
         # fcs[0..2], Wgs/Wqs/Wks/Wvs[0..3] (roi_box_feature_extractors.py:305-328)
-        _linear(sd, fe + "fcs.0.", 1024, 2048 * 49, gen)
-        for i in (1, 2):
+        _linear(sd, fe + "fcs.0.", 1024, (256 if reduce_channel else 2048) * 49, gen)
+        for i in (1, 2)[:1 + advanced_stage]:
             _linear(sd, fe + "fcs.%d." % i, 1024, 1024, gen)
-        for i in range(4):
+        for i in range(4 if advanced_stage else 2):
             sd[fe + "Wgs.%d.weight" % i] = torch.randn(16, 64, 1, 1, generator=gen) * 0.2
             sd[fe + "Wgs.%d.bias" % i] = torch.rand(16, generator=gen) * 0.5
             _linear(sd, fe + "Wqs.%d." % i, 1024, 1024, gen)
@@ -159,7 +166,7 @@ def make_state_dict(arch="mega_r101", seed=0, num_classes=31):
             sd[fe + "Wvs.%d.weight" % i] = torch.randn(1024, 1024, 1, 1, generator=gen) * (0.5 / 32)
             sd[fe + "Wvs.%d.bias" % i] = torch.randn(1024, generator=gen) * 0.01
     else:
-        _linear(sd, fe + "l_fcs.0.", 1024, 2048 * 49, gen)
+        _linear(sd, fe + "l_fcs.0.", 1024, (256 if reduce_channel else 2048) * 49, gen)
         for i in (1, 2):
             _linear(sd, fe + "l_fcs.%d." % i, 1024, 1024, gen)
         for i in range(3):
@@ -171,15 +178,18 @@ def make_state_dict(arch="mega_r101", seed=0, num_classes=31):
             sd[fe + "l_Wvs.%d.bias" % i] = torch.randn(1024, generator=gen) * 0.01
         for i in range(3):
             sd[fe + "l_us.%d" % i] = torch.randn(16, 1, 64, generator=gen) * 0.1
-        for i in range(2):
+        for i in range(global_res_stage + 1):
             _linear(sd, fe + "g_Wqs.%d." % i, 1024, 1024, gen)
             _linear(sd, fe + "g_Wks.%d." % i, 1024, 1024, gen)
             sd[fe + "g_Wvs.%d.weight" % i] = torch.randn(1024, 1024, 1, 1, generator=gen) * (0.5 / 32)
             sd[fe + "g_Wvs.%d.bias" % i] = torch.randn(1024, generator=gen) * 0.01
-        for i in range(2):
+        for i in range(global_res_stage + 1):
             sd[fe + "g_us.%d" % i] = torch.randn(16, 1, 64, generator=gen) * 0.1
     _linear(sd, "roi_heads.box.predictor.cls_score.", num_classes, 1024, gen, std=0.03)
     _linear(sd, "roi_heads.box.predictor.bbox_pred.", num_classes * 4, 1024, gen, std=0.01)
+    if reduce_channel and method in ("mega", "rdn"):
+        sd[fe + "conv.weight"] = _kaiming((256, 2048, 1, 1), gen, gain=1.0)
+        sd[fe + "conv.bias"] = torch.zeros(256)
     sd.pop("rpn.anchor_generator.cell_anchors.0")
     return sd
 

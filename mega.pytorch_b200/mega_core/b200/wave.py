@@ -138,17 +138,15 @@ class WavefrontMixin:
 
     def _wave_d(self, im_w, im_h):
         """stage 2, the rest of the group's increments (own frame included: read, then push), G1, predictor, detections"""
-        KP, R, nl12 = self.KP, self.R, self.nl12
+        KP = self.KP
         kcnt, mv = self.cur_cnt.view(-1)[:1], self._tab("mvalid")
         self._wave_apply(2, "pre", self.Y2M, self.B2)
-        self._attention(self.att_l[2], self.Y2M[:KP], KP, self.Y2M[KP:], nl12 + self.mem_cap12, self.ld_12, self.X3,
-                        boxes_q=self.Bq0[:KP], boxes_k=self.B2, m_valid=mv[2:3])
+        self._stage2(mv)
         self._wave_apply(0, "post", self.E0, self.B0)
         self._wave_apply(1, "post", self.Y1E, self.B1)
         self._wave_apply(2, "post", self.Y2M, self.B2)
-        self._attention(self.att_g[1], self.X3, KP, self.glob_x, self.GF * R, self.ld_g, self.X4,
-                        tail=lambda: self.predict_gemm(self.X4))
-        return self.predict_and_postprocess(self.X4, self.Bq0[:KP], kcnt, im_w, im_h, gemm_done=True)
+        x = self._global_res()
+        return self.predict_and_postprocess(x, self.Bq0[:KP], kcnt, im_w, im_h, gemm_done=True)
 
     def _wave(self, imgs, im_w, im_h, rank, world, payload=None):
         """generator of one wavefront step of rank `rank`: yields (tensor to all-gather, gathered output buffer) four

@@ -52,8 +52,9 @@ def vid_config(method="mega", conv_body="R-101-C4", device="cuda", num_groups=1,
 
 
 def build_detection_model_from_state_dict(sd, method="mega", device="cuda", precision=None):
-    """convenience for benchmarks/tests: infer the conv body (depth, ResNeXt groups and width) from the state dict,
-    build, load, eval"""
+    """convenience for benchmarks/tests: infer the conv body (depth, ResNeXt groups and width), REDUCE_CHANNEL, MEGA's
+    GLOBAL.RES_STAGE and RDN's ADVANCED_STAGE from the state dict, build, load, eval"""
+    fe = "roi_heads.box.feature_extractor."
     n3 = 0
     while ("backbone.body.layer3.%d.conv1.weight" % n3) in sd:
         n3 += 1
@@ -63,8 +64,13 @@ def build_detection_model_from_state_dict(sd, method="mega", device="cuda", prec
                      width_per_group=w2.shape[1])
     if precision is not None:
         cfg.MODEL.B200.PRECISION = precision
-    if method == "base" and "roi_heads.box.feature_extractor.conv.weight" not in sd:
-        cfg.MODEL.VID.ROI_BOX_HEAD.REDUCE_CHANNEL = False
+    cfg.MODEL.VID.ROI_BOX_HEAD.REDUCE_CHANNEL = (fe + "conv.weight") in sd
+    count = lambda name: sum(1 for k in sd if k.startswith(fe + name) and k.endswith(".weight"))     # noqa: E731
+    if method == "mega":
+        cfg.MODEL.VID.MEGA.GLOBAL.RES_STAGE = count("g_Wqs.") - 1
+    elif method == "rdn":
+        att = cfg.MODEL.VID.ROI_BOX_HEAD.ATTENTION
+        att.ADVANCED_STAGE = 0 if count("Wqs.") == att.STAGE else 1
     model = build_detection_model(cfg)
     if body is None:
         model.adopt_state_dict(sd)          # non-standard depth (tests): skip the module tree, feed the engine

@@ -186,17 +186,22 @@ def _fc(i, o):
     return nn.Linear(i, o)
 
 
+def _reduce_channel(extractor, cfg):
+    """MODEL.VID.ROI_BOX_HEAD.REDUCE_CHANNEL (roi_box_feature_extractors.py:274-283, :474-483): a 1x1 conv 2048 -> 256
+    (+ ReLU) between res5 and ROIAlign as `extractor.conv`; returns the channel count ROIAlign pools"""
+    if cfg.MODEL.VID.ROI_BOX_HEAD.REDUCE_CHANNEL:
+        extractor.conv = nn.Conv2d(2048, 256, 1)
+        return 256
+    extractor.conv = None
+    return 2048
+
+
 @registry.ROI_BOX_FEATURE_EXTRACTORS.register("ResNetConv52MLPFeatureExtractor")
 class ResNetConv52MLPFeatureExtractor(nn.Module):
     def __init__(self, cfg, in_channels):
         super().__init__()
         self.head = ResNetHead(cfg)
-        ch = 2048
-        if cfg.MODEL.VID.ROI_BOX_HEAD.REDUCE_CHANNEL:
-            self.conv = nn.Conv2d(2048, 256, 1)
-            ch = 256
-        else:
-            self.conv = None
+        ch = _reduce_channel(self, cfg)
         res = cfg.MODEL.ROI_BOX_HEAD.POOLER_RESOLUTION
         dim = cfg.MODEL.ROI_BOX_HEAD.MLP_HEAD_DIM
         self.fc6 = _fc(ch * res * res, dim)
@@ -237,12 +242,12 @@ class MEGAFeatureExtractor(_WindowedExtractorForward, nn.Module):
     def __init__(self, cfg, in_channels):
         super().__init__()
         self.head = ResNetHead(cfg)
-        self.conv = None
+        ch = _reduce_channel(self, cfg)
         res = cfg.MODEL.ROI_BOX_HEAD.POOLER_RESOLUTION
         dim = cfg.MODEL.ROI_BOX_HEAD.MLP_HEAD_DIM
         att = cfg.MODEL.VID.ROI_BOX_HEAD.ATTENTION
         emb, grp, stages = att.EMBED_DIM, att.GROUP, att.STAGE
-        self.l_fcs = nn.ModuleList([_fc(2048 * res * res if i == 0 else dim, dim) for i in range(stages)])
+        self.l_fcs = nn.ModuleList([_fc(ch * res * res if i == 0 else dim, dim) for i in range(stages)])
         self.l_Wgs = nn.ModuleList([nn.Conv2d(emb, grp, 1) for _ in range(stages)])
         self.l_Wqs = nn.ModuleList([_fc(dim, dim) for _ in range(stages)])
         self.l_Wks = nn.ModuleList([_fc(dim, dim) for _ in range(stages)])
@@ -263,14 +268,14 @@ class RDNFeatureExtractor(_WindowedExtractorForward, nn.Module):
     def __init__(self, cfg, in_channels):
         super().__init__()
         self.head = ResNetHead(cfg)
-        self.conv = None
+        ch = _reduce_channel(self, cfg)
         res = cfg.MODEL.ROI_BOX_HEAD.POOLER_RESOLUTION
         dim = cfg.MODEL.ROI_BOX_HEAD.MLP_HEAD_DIM
         att = cfg.MODEL.VID.ROI_BOX_HEAD.ATTENTION
         emb, grp, base, adv = att.EMBED_DIM, att.GROUP, att.STAGE, att.ADVANCED_STAGE
         n_att = base if adv == 0 else base + adv + 1
         n_fc = base if adv == 0 else base + adv
-        self.fcs = nn.ModuleList([_fc(2048 * res * res if i == 0 else dim, dim) for i in range(n_fc)])
+        self.fcs = nn.ModuleList([_fc(ch * res * res if i == 0 else dim, dim) for i in range(n_fc)])
         self.Wgs = nn.ModuleList([nn.Conv2d(emb, grp, 1) for _ in range(n_att)])
         self.Wqs = nn.ModuleList([_fc(dim, dim) for _ in range(n_att)])
         self.Wks = nn.ModuleList([_fc(dim, dim) for _ in range(n_att)])
@@ -380,10 +385,22 @@ def engine_config_from(cfg):
     if any(m.RESNETS.STAGE_WITH_DCN):
         unsupported.append("MODEL.RESNETS.STAGE_WITH_DCN = %s (the engines have no deformable backbone stages)"
                            % (tuple(m.RESNETS.STAGE_WITH_DCN),))
+    att = v.ROI_BOX_HEAD.ATTENTION
     if v.METHOD == "mega":
         if not (v.MEGA.MEMORY.ENABLE and v.MEGA.GLOBAL.ENABLE):
             unsupported.append("MODEL.VID.MEGA.MEMORY.ENABLE / GLOBAL.ENABLE = False (MegaEngine is laid out for memory + "
                                "global aggregation, generalized_rcnn_mega.py:36-40)")
+        if att.STAGE != 3:
+            unsupported.append("MODEL.VID.ROI_BOX_HEAD.ATTENTION.STAGE = %d (MegaEngine runs 3 local stages)" % att.STAGE)
+        if v.MEGA.GLOBAL.RES_STAGE not in (0, 1):
+            unsupported.append("MODEL.VID.MEGA.GLOBAL.RES_STAGE = %d (MegaEngine runs 0 or 1 global stages after the "
+                               "local ones)" % v.MEGA.GLOBAL.RES_STAGE)
+    if v.METHOD == "rdn":
+        if att.STAGE != 2:
+            unsupported.append("MODEL.VID.ROI_BOX_HEAD.ATTENTION.STAGE = %d (RdnEngine runs 2 base stages)" % att.STAGE)
+        if att.ADVANCED_STAGE not in (0, 1):
+            unsupported.append("MODEL.VID.ROI_BOX_HEAD.ATTENTION.ADVANCED_STAGE = %d (RdnEngine runs 0 or 1 advanced "
+                               "stages)" % att.ADVANCED_STAGE)
     if unsupported:
         raise NotImplementedError("mega_core (B200 build): " + "; ".join(unsupported))
     # the reference sizes the long-range memory deques with ALL_FRAME_INTERVAL (roi_box_feature_extractors.py:660-668:
