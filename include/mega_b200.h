@@ -58,7 +58,9 @@ typedef struct mega_conv_gemm_desc {
   int taps_r, taps_s, dil, pad;
   int k_per_tap; /* reduction length per tap (Cin) */
   /* output NHWC, dense in (w, h, n) with out_ld elements between pixels (written by TMA: 16-byte aligned
-   * base and pitch; the residual likewise, same element type as the output); out_h/out_w = output spatial size */
+   * base and pitch; the residual likewise, same element type as the output); out_h/out_w = output spatial size. Nothing
+   * outside the output view changes: not the channels past cout + (batch - 1) * out_c_off (split-fp16 outputs: cout rounded
+   * up to 32), whatever the row pitch */
   void* out;
   long long out_ld;
   int n_img, out_h, out_w, cout;

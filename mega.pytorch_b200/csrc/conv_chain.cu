@@ -302,8 +302,10 @@ __device__ __forceinline__ void chain_epilogue_layer(const ChainLayer* L, const 
         }
         fence_async_smem();
         __syncwarp();
-        if (lane == 0) {
-          tma_store_4d(tmOut, smem + kChainEpiOffset + ew * 8192, nb + tc.batch * p.out_c_off, box.w, box.h, out_n);
+        const int gc0 = nb + tc.batch * p.out_c_off;
+        if (gc0 + CW > p.out_tail0) store_tail<OUT16>(p, smem + kChainEpiOffset + ew * 8192 + lane * 128, gc0, CW, box, out_n, lane);
+        if (lane == 0 && gc0 < p.out_tail0) {
+          tma_store_4d(tmOut, smem + kChainEpiOffset + ew * 8192, gc0, box.w, box.h, out_n);
           tma_store_commit();
         }
       }

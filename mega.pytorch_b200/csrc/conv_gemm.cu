@@ -191,6 +191,8 @@ int encode_conv_gemm_problem(const mega_conv_gemm_desc* d, CUtensorMap* tmA_p, C
   // pixels), 128B swizzle
   CUtensorMap& tmOut = *tmOut_p;
   CUtensorMap& tmRes = *tmRes_p;
+  int out_cext = 0, out_tail0 = 0;
+  long long out_str_h = 0, out_str_n = 0;
   {
     const int box_w = d->tile_w < 32 ? d->tile_w : 32;
     const int box_h = 32 / box_w;
@@ -206,8 +208,16 @@ int encode_conv_gemm_problem(const mega_conv_gemm_desc* d, CUtensorMap* tmA_p, C
       const int c_off = which == 0 ? d->out_c_off : d->res_c_off;
       const int n_off = which == 0 ? d->out_n_off : d->res_n_off;
       const bool split_fmt = pk && (which == 0 ? d->out_f16 != 0 : d->res_split != 0);
-      const int c_extent = split_fmt ? ((d->cout + 31) & ~31) : d->cout;
-      cuuint64_t gdim[4] = {static_cast<cuuint64_t>(c_extent + (d->batch - 1) * c_off), static_cast<cuuint64_t>(d->out_w),
+      const int c_extent = (split_fmt ? ((d->cout + 31) & ~31) : d->cout) + (d->batch - 1) * c_off;
+      // the store's channel extent ends at the last 16-byte boundary (the TMA unit clips stores at 16-byte granularity);
+      // the epilogue writes the rest of the row with plain stores (ConvGemmParams::out_tail0)
+      const int c_tail0 = (c_extent * osz / 16) * 16 / osz;
+      if (which == 0) {
+        out_cext = c_extent;
+        out_tail0 = c_tail0;
+      }
+      const int c_map = (which == 0 && c_tail0 > 0) ? c_tail0 : c_extent;
+      cuuint64_t gdim[4] = {static_cast<cuuint64_t>(c_map), static_cast<cuuint64_t>(d->out_w),
                             static_cast<cuuint64_t>(d->out_h),
                             static_cast<cuuint64_t>(d->n_img + (d->batch - 1) * n_off)};
       const long long sh = which == 0 ? d->out_stride_h : d->res_stride_h;
@@ -215,6 +225,10 @@ int encode_conv_gemm_problem(const mega_conv_gemm_desc* d, CUtensorMap* tmA_p, C
       const long long str_h = sh > 0 ? sh : ld * d->out_w;
       const long long str_n = sn > 0 ? sn : str_h * d->out_h;
       MEGA_ARG_CHECK((str_h % oalign) == 0 && (str_n % oalign) == 0, "conv_gemm: output strides must be multiples of 16 bytes");
+      if (which == 0) {
+        out_str_h = str_h;
+        out_str_n = str_n;
+      }
       cuuint64_t gstr[3] = {static_cast<cuuint64_t>(ld) * osz, static_cast<cuuint64_t>(str_h) * osz,
                             static_cast<cuuint64_t>(str_n) * osz};
       cuuint32_t box[4] = {static_cast<cuuint32_t>(cw), static_cast<cuuint32_t>(box_w), static_cast<cuuint32_t>(box_h), 1};
@@ -274,6 +288,12 @@ int encode_conv_gemm_problem(const mega_conv_gemm_desc* d, CUtensorMap* tmA_p, C
   p.b_lo_tap_off = d->b_lo_tap_off;
   p.res_split = d->res_split ? 1 : 0;
   p.acc_scale = (pk && d->acc_scale != 0.f) ? d->acc_scale : 1.f;
+  p.out_ptr = d->out;
+  p.out_ld = d->out_ld;
+  p.out_str_h = out_str_h;
+  p.out_str_n = out_str_n;
+  p.out_tail0 = out_tail0;
+  p.out_cext = out_cext;
   MEGA_ARG_CHECK(tiles <= kCounterSlots, "conv_gemm: %lld output tiles exceed the %d counter slots", tiles, kCounterSlots);
   MEGA_ARG_CHECK(p.total_units > 0, "conv_gemm: empty problem");
   MEGA_ARG_CHECK(p.total_units * kMaxCtas < (1LL << 31), "conv_gemm: %lld work units exceed the 32-bit work-list range",

@@ -89,6 +89,12 @@ struct ConvGemmParams {
   int res_split;             // 3xFP16 only: the residual tensor is in the split-fp16 format (else fp32)
   float acc_scale;           // 3xFP16 only: the accumulator is multiplied by this power of two first (weights are stored
                              // scaled by its inverse so that their low halves stay normal fp16 numbers)
+  // The TMA unit clips a store's innermost (channel) extent at 16-byte granularity. tmOut therefore ends at out_tail0, the
+  // last 16-byte boundary at or before the channel extent out_cext; the channels [out_tail0, out_cext) of a pixel are
+  // written with plain stores (store_tail), so that nothing past out_cext changes.
+  void* out_ptr;
+  long long out_ld, out_str_h, out_str_n;   // element strides of the output pixels / rows / images
+  int out_tail0, out_cext;
 };
 
 template <int BN, int STAGES, int MODE = kModeTf32>
@@ -247,6 +253,27 @@ __device__ __forceinline__ StoreBox store_box(const ConvGemmParams& p, const Til
   const int r0 = q * 32;
   const int bh0 = r0 / p.tile_w, bw0 = r0 - bh0 * p.tile_w;
   return {tc.w0 + bw0, tc.h0 + bh0, tc.img + tc.batch * p.res_n_off};
+}
+
+// Channels [out_tail0, out_cext) of this lane's pixel that fall in a staged output chunk (128-byte swizzled row `rowp`,
+// global channel gc0 at its column 0, cw columns): plain stores of what the TMA store would clip at 16-byte granularity.
+template <bool HALF>
+__device__ __forceinline__ void store_tail(const ConvGemmParams& p, const uint8_t* rowp, int gc0, int cw, const StoreBox& box,
+                                          int out_n, int lane) {
+  const int h = box.h + lane / p.box_w, w = box.w + lane % p.box_w;
+  if (h >= p.out_h || w >= p.out_w) return;
+  const int j0 = max(p.out_tail0 - gc0, 0), j1 = min(p.out_cext - gc0, cw);
+  const uint32_t sw = static_cast<uint32_t>(lane & 7);
+  const long long pix = static_cast<long long>(out_n) * p.out_str_n + static_cast<long long>(h) * p.out_str_h +
+                        static_cast<long long>(w) * p.out_ld + gc0;
+  for (int j = j0; j < j1; ++j) {
+    if (HALF)
+      static_cast<uint16_t*>(p.out_ptr)[pix + j] =     // fp16 bits
+          *reinterpret_cast<const uint16_t*>(rowp + ((static_cast<uint32_t>(j >> 3) ^ sw) << 4) + (j & 7) * 2);
+    else
+      static_cast<float*>(p.out_ptr)[pix + j] =
+          *reinterpret_cast<const float*>(rowp + ((static_cast<uint32_t>(j >> 2) ^ sw) << 4) + (j & 3) * 4);
+  }
 }
 
 // Column i of the tile's scale / bias slice into shared memory (scale at sb, bias at sb + bias_off), so that the chunk loops
@@ -869,8 +896,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
             fence_async_smem();
             __syncwarp();
-            if (lane == 0) {
-              tma_store_4d(&tmOut, stage_buf + j * 4096, tc.n0 + cj * 32 + tc.batch * p.out_c_off, box.w, box.h, out_n);
+            const int gc0 = tc.n0 + cj * 32 + tc.batch * p.out_c_off;
+            if (!OUT16 && gc0 + 32 > p.out_tail0) store_tail<false>(p, rowp, gc0, 32, box, out_n, lane);
+            if (lane == 0 && gc0 < p.out_tail0) {
+              tma_store_4d(&tmOut, stage_buf + j * 4096, gc0, box.w, box.h, out_n);
               tma_store_commit();
             }
           } else if (complete) {
@@ -1017,8 +1046,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
           fence_async_smem();
           __syncwarp();
-          if (lane == 0) {
-            tma_store_4d(&tmOut, epi_out + (c & 1) * 4096, nb + tc.batch * p.out_c_off, box.w, box.h, out_n);
+          const int gc0 = nb + tc.batch * p.out_c_off;
+          if (gc0 + CW > p.out_tail0) store_tail<OUTH>(p, dst, gc0, CW, box, out_n, lane);
+          if (lane == 0 && gc0 < p.out_tail0) {
+            tma_store_4d(&tmOut, epi_out + (c & 1) * 4096, gc0, box.w, box.h, out_n);
             tma_store_commit();
           }
         };
