@@ -431,6 +431,34 @@ int mega_vid_match_host(const float* pred_boxes, int n_pred, const float* gt_box
                         int n_gt, float iou_thresh, double empty_weight, signed char* match_out,
                         double* pred_ignore_out);
 
+/* ---------------------------------------------------------------- Seq-NMS over whole videos
+ * Sequence-level post-processing of the detections of whole videos (Han et al., "Seq-NMS for Video Object Detection",
+ * arXiv:1602.08465). No reference counterpart: the reference ships none; this runs after the per-frame detections of
+ * tools/test_net.py and before VID evaluation (mega_core.engine.seq_nms).
+ * Input, packed per frame (F frames of num_videos videos, video v = frames [video_offsets[v], video_offsets[v+1])):
+ * boxes [F, max_det, 4] xyxy fp32 (16-byte aligned), scores [F, max_det], labels [F, max_det] int32, counts [F]; the
+ * first counts[f] slots of frame f are its detections with labels in ASCENDING order (class-major, as the engines return
+ * them); other slots are ignored. video_offsets [num_videos + 1], ascending, 0 <= ... <= F (device memory). For each
+ * video and each class c in [0, num_classes) independently:
+ *   1. box i of frame t links to box j of frame t+1 (same video, same class) iff IoU(i, j) > link_iou ("+1" pixel
+ *      convention, fp32, decided as RN(inter / union) > thresh exactly like mega_nms);
+ *   2. over the boxes still alive: best[t][i] = score[t][i] + (max of best[t+1][j] over alive linked j, or 0), in fp64;
+ *      the successor of i is the linked j of largest best (ties: smallest j); the root is the alive box of largest best
+ *      (ties: smallest t, then smallest slot); the chain is the root followed by its successors;
+ *   3. every chain box gets the score (float)(best[root] / length) (rescore 0, "avg"; best[root] is the chain's score
+ *      sum accumulated from its last frame backward) or the chain's largest score (rescore 1, "max") and is selected;
+ *   4. in each frame of the chain, every alive box with IoU(box, chain box) > nms_iou is suppressed;
+ *   5. repeat from 2 until no box of the class is alive.
+ * Output: keep [F, max_det] uint8 = 1 for the selected boxes, out_scores [F, max_det] their new scores (0 elsewhere).
+ * Deterministic (no result depends on scheduling). max_det <= 512. workspace: >= mega_seq_nms_workspace_bytes(F,
+ * max_det, num_classes) bytes, 256-byte aligned, no initialisation needed; mega_seq_nms_workspace_bytes returns -1 for
+ * arguments out of range. */
+long long mega_seq_nms_workspace_bytes(int num_frames, int max_det, int num_classes);
+int mega_seq_nms(const float* boxes, const float* scores, const int* labels, const int* counts, int num_frames,
+                 int max_det, const int* video_offsets, int num_videos, int num_classes, float link_iou, float nms_iou,
+                 int rescore, void* workspace, long long workspace_bytes, float* out_scores, unsigned char* keep,
+                 void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -952,6 +952,42 @@ def box_postprocess(logits, deltas, proposals, count, num_classes, im_w, im_h, s
     return out
 
 
+SEQ_NMS_RESCORE = {"avg": 0, "max": 1}
+
+
+def seq_nms_workspace_bytes(num_frames, max_det, num_classes):
+    nbytes = lib.mega_seq_nms_workspace_bytes(num_frames, max_det, num_classes)
+    if nbytes < 0:
+        raise _lib.MegaError("seq_nms: %d frames of at most %d detections, %d classes: out of range (max_det <= 512)"
+                             % (num_frames, max_det, num_classes))
+    return nbytes
+
+
+def seq_nms(boxes, scores, labels, counts, video_offsets, num_classes, link_iou=0.5, nms_iou=0.3, rescore="avg"):
+    """Seq-NMS of several videos in one launch (include/mega_b200.h, mega_seq_nms). boxes [F, D, 4] fp32, scores [F, D],
+    labels [F, D] int32 ascending inside each frame's first counts[f] slots, counts [F] int32, video_offsets [V+1] int32.
+    Returns (new scores [F, D] fp32, keep [F, D] uint8) on the device; no synchronisation."""
+    require_cuda(boxes, scores, labels, counts, video_offsets)
+    if rescore not in SEQ_NMS_RESCORE:
+        raise ValueError("seq_nms: rescore must be one of %s, got %r" % (sorted(SEQ_NMS_RESCORE), rescore))
+    f, d = scores.shape
+    boxes = boxes.contiguous().float()
+    scores = scores.contiguous().float()
+    labels = labels.contiguous().int()
+    counts = counts.contiguous().int()
+    video_offsets = video_offsets.contiguous().int()
+    nbytes = seq_nms_workspace_bytes(f, d, num_classes)
+    ws = _workspace("seq_nms", nbytes, boxes.device)
+    out_scores = torch.empty(f, d, dtype=torch.float32, device=boxes.device)
+    keep = torch.empty(f, d, dtype=torch.uint8, device=boxes.device)
+    check(lib.mega_seq_nms(ptr(boxes), ptr(scores), ptr(labels), ptr(counts), f, d, ptr(video_offsets),
+                           video_offsets.numel() - 1, int(num_classes), float(link_iou), float(nms_iou),
+                           SEQ_NMS_RESCORE[rescore], ptr(ws), ws.numel(), ptr(out_scores), ptr(keep), stream_ptr()),
+          "mega_seq_nms")
+    LAUNCHES[0] += 3
+    return out_scores, keep
+
+
 # --------------------------------------------------------------------------- FGFA helpers (csrc/fgfa.cu)
 def _is16(t):
     return 1 if t.dtype == torch.float16 else 0

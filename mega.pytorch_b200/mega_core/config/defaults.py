@@ -127,7 +127,11 @@ _C = CfgNode({
                          "REF_NUM": 2}},
         # B200 build only: arithmetic of the tensor-core contractions -- "f16" (fp16 operands / storage, throughput
         # mode), "tf32" (fp32 storage, TF32 operands), "fp32x3" (3xTF32 split, strict parity with the fp32 reference)
-        "B200": {"PRECISION": "f16"},
+        # SEQ_NMS (B200 build only): Seq-NMS over whole videos after the detection loop (mega_core.engine.seq_nms) --
+        # boxes of consecutive frames link at IoU > LINK_IOU, a chain suppresses IoU > NMS_IOU in its frames, its boxes
+        # get the chain's "avg" or "max" score
+        "B200": {"PRECISION": "f16",
+                 "SEQ_NMS": {"ENABLED": False, "LINK_IOU": 0.5, "NMS_IOU": 0.3, "RESCORE": "avg"}},
     },
     "INPUT": {"MIN_SIZE_TRAIN": (800,), "MAX_SIZE_TRAIN": 1333, "MIN_SIZE_TEST": 800, "MAX_SIZE_TEST": 1333,
               "PIXEL_MEAN": [102.9801, 115.9465, 122.7717], "PIXEL_STD": [1.0, 1.0, 1.0], "TO_BGR255": True},

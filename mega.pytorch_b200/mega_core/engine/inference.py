@@ -13,6 +13,7 @@ import torch
 
 from ..data.datasets.evaluation.vid import vid_evaluation
 from ..utils.comm import gather_predictions, get_world_size, is_main_process, synchronize
+from .seq_nms import seq_nms_predictions
 
 
 class Timer(object):
@@ -69,6 +70,28 @@ def _seconds(t):
     return time.strftime("%H:%M:%S", time.gmtime(t))
 
 
+def _seq_nms_kwargs(settings):
+    """MODEL.B200.SEQ_NMS (a CfgNode, or a dict with its keys ENABLED / LINK_IOU / NMS_IOU / RESCORE) -> keyword
+    arguments of seq_nms_predictions, or None when absent or not enabled"""
+    if settings is None:
+        return None
+    get = settings.get if isinstance(settings, dict) else lambda k, d=None: getattr(settings, k, d)
+    if not get("ENABLED", False):
+        return None
+    return {"link_iou": float(get("LINK_IOU", 0.5)), "nms_iou": float(get("NMS_IOU", 0.3)),
+            "rescore": str(get("RESCORE", "avg"))}
+
+
+def _apply_seq_nms(predictions, dataset, kwargs, world, logger):
+    """Seq-NMS over the videos of `predictions` ({image_id: BoxList}); logged like the other timings"""
+    t0 = time.time()
+    predictions = seq_nms_predictions(predictions, dataset, **kwargs)
+    t = time.time() - t0
+    logger.info("Seq-NMS time: {} ({} s / img per device, on {} devices)".format(
+        _seconds(t), t * world / max(len(dataset), 1), world))
+    return predictions
+
+
 def inference(cfg, model, data_loader, dataset_name, iou_types=("bbox",), motion_specific=False, box_only=False,
               bbox_aug=False, device="cuda", expected_results=(), expected_results_sigma_tol=4, output_folder=None):
     """engine/inference.py:72-134; VID datasets only (`dataset` needs get_img_info / get_groundtruth /
@@ -86,6 +109,10 @@ def inference(cfg, model, data_loader, dataset_name, iou_types=("bbox",), motion
     logger.info("Total run time: {} ({} s / img per device, on {} devices)".format(_seconds(t), t * world / len(dataset), world))
     logger.info("Model inference time: {} ({} s / img per device, on {} devices)".format(
         _seconds(model_only.total_time), model_only.total_time * world / len(dataset), world))
+    # per rank, before the gather: VIDTestDistributedSampler gives every rank whole videos
+    seq = _seq_nms_kwargs(getattr(getattr(cfg.MODEL, "B200", None), "SEQ_NMS", None))
+    if seq is not None:
+        predictions = _apply_seq_nms(predictions, dataset, seq, world, logger)
     predictions = gather_predictions(predictions)
     if not is_main_process():
         return None
@@ -97,8 +124,15 @@ def inference(cfg, model, data_loader, dataset_name, iou_types=("bbox",), motion
 
 
 def inference_no_model(data_loader, iou_types=("bbox",), motion_specific=False, box_only=False, expected_results=(),
-                       expected_results_sigma_tol=4, output_folder=None):
-    """engine/inference.py:137-160: score the predictions.pth of an earlier run"""
+                       expected_results_sigma_tol=4, output_folder=None, seq_nms=None):
+    """engine/inference.py:137-160: score the predictions.pth of an earlier run. `seq_nms`: a dict with the keys of
+    MODEL.B200.SEQ_NMS (ENABLED, LINK_IOU, NMS_IOU, RESCORE), e.g. dict(cfg.MODEL.B200.SEQ_NMS), to rescore the saved
+    predictions with Seq-NMS first (the file is not changed)"""
     predictions = torch.load(os.path.join(output_folder, "predictions.pth"), weights_only=False)
+    seq = _seq_nms_kwargs(seq_nms)
+    if seq is not None:
+        by_id = _apply_seq_nms(dict(enumerate(predictions)), data_loader.dataset, seq, 1,
+                               logging.getLogger("mega_core.inference"))
+        predictions = [by_id[i] for i in range(len(predictions))]
     return vid_evaluation(dataset=data_loader.dataset, predictions=predictions, output_folder=output_folder,
                           box_only=box_only, motion_specific=motion_specific)
