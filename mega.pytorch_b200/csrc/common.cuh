@@ -168,6 +168,21 @@ __device__ __forceinline__ void wgmma_wait_regs(float (&d)[N]) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Per-warpgroup register budget: every warp of the warpgroup executes the same call. dec hands registers back to the
+// CTA's pool; inc waits until the pool holds enough (the decs of the other warpgroups) and ptxas allocates the code that
+// follows within the new count.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+// blockIdx.x read where it is used (volatile: not merged with an earlier read). After setmaxnreg, ptxas keeps a value that
+// lives from the kernel's prologue into the regions of different register counts in local memory.
+__device__ __forceinline__ int ctaid_x_here() {
+  int r;
+  asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(r));
+  return r;
+}
+
 // K-major operand tile stored as rows of exactly 128 bytes with the 128B swizzle
 // (what TMA writes for a box whose inner extent is 128 B): 8-row groups are 1024 B apart.
 // Advancing the start address by 32 B selects the next 32 bytes of K inside the swizzle row.

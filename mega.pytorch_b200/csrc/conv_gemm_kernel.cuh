@@ -13,10 +13,15 @@
 // Tiling: the M tile is a th x tw rectangle of 128 output pixels, so the A operand of filter
 // tap (r,s) is the same rectangle shifted by (r,s)*dilation - pad: a plain 4-D tiled TMA load
 // with out-of-bounds zero fill supplies the padding. K is consumed in slabs of 32 floats
-// (= one 128 B swizzle row) per tap. Warp roles: warp 0 TMA producer, warps 2-5 epilogue (accumulator ring -> registers
-// -> global); the strict modes add warps 6-9: operand splitters (3xTF32) or a second set of epilogue warps (3xFP16 on
-// split-fp16 tensors, the mode the strict engine runs; see kModeF16x3 below). Two MMA warpgroups follow the last of these
-// warps (kMmaWarp0): warpgroup g issues the wgmma of tile rows [64 g, 64 g + 64) and keeps that accumulator in registers.
+// (= one 128 B swizzle row) per tap. Warp roles: warp 0 TMA producer, warp 1 barrier init, warps 2-5 epilogue
+// (accumulator ring -> registers -> global); 3xTF32 adds warps 6-9, the operand splitters. Two MMA warpgroups follow the
+// last of these warps (kMmaWarp0): warpgroup g issues the wgmma of tile rows [64 g, 64 g + 64) and keeps that accumulator
+// in registers.
+// 3xFP16 (split-fp16 tensors, the mode the strict engine runs; see kModeF16x3 below) keeps each role in whole warpgroups
+// and moves registers between them with setmaxnreg (512 threads start at 128 registers each): warpgroup 0 (warps 0-3:
+// producer, barrier init, two idle warps) drops to 40, warpgroup 1 (warps 4-7: the epilogue) to 104, and the two MMA
+// warpgroups (warps 8-15) rise to 184, so that the wgmma accumulator and the round-to-nearest master accumulator (64 + 64
+// registers per thread at block_n 128) stay in registers.
 #include "common.cuh"
 #pragma once
 #include "mega_b200.h"
@@ -37,17 +42,20 @@ constexpr int kModeF16x3 = 3;   // "3xFP16": operands stored SPLIT in HBM -- eve
 // every mode stages K slabs of 128 bytes per row (one swizzle row) and issues 4 MMAs of 32 bytes of K each
 // (3xFP16: 2 k-steps x 3 products over the hi / lo halves of the row; 3xTF32: 4 k-steps x 3 products)
 __host__ __device__ constexpr int mode_bk(int mode) { return mode == kModeF16 ? 64 : 32; }
-constexpr int kThreads = 192;   // 6 warps before the MMA warpgroups (10 in the strict modes)
+constexpr int kThreads = 192;   // 6 warps before the MMA warpgroups (10 in the 3xTF32 mode)
 constexpr int kMaxCtas = 132;   // persistent grid: one CTA per SM of an H100 SXM
 // The MMA warpgroups hand finished accumulators to the epilogue warps through a ring of shared-memory slots of 32 columns
 // x 128 rows fp32 (row r = 128 bytes, 16-byte groups swizzled by r & 7: conflict-free for both sides). Every slot is read by
 // four epilogue warps (one per 32-row quarter) and produced in column order, tile after tile.
 constexpr int kRingSlots = 2;
 constexpr int kRingSlotBytes = kBM * 128;
-__host__ __device__ constexpr int mma_warp0(int mode) {
-  return (mode == kModeSplit3 || mode == kModeF16x3) ? 12 : 8;
-}
+__host__ __device__ constexpr int mma_warp0(int mode) { return mode == kModeSplit3 ? 12 : 8; }
 __host__ __device__ constexpr int conv_gemm_threads(int mode) { return (mma_warp0(mode) + 8) * 32; }
+// 3xFP16 registers per thread of warpgroup 0 (producer), 1 (epilogue) and 2-3 (MMA): the 64K registers of the SM
+constexpr int kF16x3RegsProducer = 40, kF16x3RegsEpilogue = 104, kF16x3RegsMma = 184;
+static_assert(128 * kF16x3RegsProducer + 128 * kF16x3RegsEpilogue + 256 * kF16x3RegsMma == 65536 &&
+                  conv_gemm_threads(kModeF16x3) == 512,
+              "3xFP16 register split");
 // An N tile wider than 128 columns is computed in two passes over the same k-blocks (columns [0, P0), then [P0, block_n)):
 // a pass keeps at most 64 accumulator registers per MMA thread. Both widths are multiples of 32 (whole ring chunks).
 __host__ __device__ constexpr int pass_n(int bn) { return bn <= 128 ? bn : (bn == 160 ? 96 : bn / 2); }
@@ -107,6 +115,7 @@ struct SmemLayout {
   static constexpr int kStageBytes = SPLIT3 ? kHalf + kBBytes : kHalf;
   static constexpr int kRingOffset = STAGES * kStageBytes;
   static constexpr int kEpiOffset = kRingOffset + kRingSlots * kRingSlotBytes;   // 4 warps x (2 out + 2 residual) x 4 KB
+                                                                                 // (3xFP16: 4 warps x 4 chunks x 4 KB)
   static constexpr int kEpiBytes = 4 * 4 * 4096;
   static constexpr int kBarOffset = kEpiOffset + kEpiBytes;
   static constexpr int kSbCols = BN <= 128 ? 128 : 256;
@@ -544,6 +553,10 @@ __device__ __forceinline__ void mma_pass(uint8_t* smem, uint64_t* full_bar, uint
   const int lane = wtid & 31;
   float d[PN / 2];
   float master[SEG ? PN / 2 : 1];
+  if constexpr (MODE == kModeF16x3) {
+#pragma unroll
+    for (int i = 0; i < PN / 2; ++i) master[i] = -0.f;
+  }
   bool has_master = false;
   for (int s0 = kb0, s1 = 0; s0 < kb1; s0 = s1) {
     s1 = (kb1 - s0 > seg_len) ? s0 + seg_len : kb1;
@@ -578,7 +591,13 @@ __device__ __forceinline__ void mma_pass(uint8_t* smem, uint64_t* full_bar, uint
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[pending]);
     }
-    if constexpr (SEG) {
+    if constexpr (MODE == kModeF16x3) {
+      // master starts at -0, and -0 + x == x for every non-NaN x (zeros and infinities included): the values the select
+      // below gives. Written as that select, the fold made ptxas build each new master beside the old one (64 + 64 + 64
+      // registers at PN = 128) and spill.
+#pragma unroll
+      for (int i = 0; i < PN / 2; ++i) master[i] = __fadd_rn(d[i], master[i]);
+    } else if constexpr (SEG) {
 #pragma unroll
       for (int i = 0; i < PN / 2; ++i) master[i] = has_master ? __fadd_rn(d[i], master[i]) : d[i];
       has_master = true;
@@ -638,7 +657,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* split_bar = empty_bar + STAGES;       // [STAGES] (3xTF32 only)
   uint64_t* ring_full = split_bar + STAGES;       // [kRingSlots]
   uint64_t* ring_empty = ring_full + kRingSlots;  // [kRingSlots]
-  uint64_t* res_bar = ring_empty + kRingSlots;    // [4 warps][2] (3xFP16: [8 warps][2])
+  uint64_t* res_bar = ring_empty + kRingSlots;    // [4 warps][2] (3xFP16: [4 warps][4 chunks])
   int* epi_flag = reinterpret_cast<int*>(res_bar + 16);
   uint8_t* ring = smem + L::kRingOffset;
 
@@ -673,9 +692,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   griddep_launch_dependents();  // let the next kernel's prologue overlap this kernel
   if (warp == 0) {
     // ===================== TMA producer =====================
+    if (PK) setmaxnreg_dec<kF16x3RegsProducer>();
     if (lane < 2) {
       PipeState ps = {0, 0};
-      WorkIter it(p, cta, grid);
+      WorkIter it(p, PK ? ctaid_x_here() : cta, grid);
       int t;
       int kb0, kb1;
       const bool b_lo = SPLIT3 && p.b_lo_tap_off > 0;    // pre-split weights: the low parts come by TMA too
@@ -689,11 +709,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   } else if (warp >= kMmaWarp0) {
     // ===================== MMA warpgroups =====================
+    if (PK) setmaxnreg_inc<kF16x3RegsMma>();
     const int wg = (warp - kMmaWarp0) >> 2;          // tile rows [64 wg, 64 wg + 64)
     const int wtid = threadIdx.x - (kMmaWarp0 + 4 * wg) * 32;
     constexpr int P0 = pass_n(BN), P1 = BN - P0;
     MmaState ms = {0, 0, {0, 0}};
-    WorkIter it(p, cta, grid);
+    WorkIter it(p, PK ? ctaid_x_here() : cta, grid);
     int t;
     int kb0, kb1;
     while (it.next(t, kb0, kb1)) {
@@ -742,23 +763,23 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp >= 2 && warp < 10 && PK) {
-    // ===================== epilogue, 3xFP16 (warps 2..9) =====================
-    // Two warps share a 32-row quarter of the tile; of its 32-column chunks each takes every other one (chunk cj = 2 j + half):
-    // every ring slot is read by the four warps of one half. The BN scale is folded into the packed weights, the bias slice
-    // of the NEXT tile is fetched during the current one (double-buffered, one barrier per tile), and the residual lands in
-    // the store staging buffer itself (every thread reads its 128-byte row into registers before it writes the same row),
-    // issued for all chunks at the start of the tile.
-    constexpr int kCPW = BN / 64;          // 32-column chunks per warp
+  } else if (PK && warp >= 4 && warp < 8) {
+    // ===================== epilogue, 3xFP16 (warps 4..7) =====================
+    // One warp per 32-row quarter of the tile finishes all of its 32-column chunks: every ring slot is read by all four
+    // warps. The BN scale is folded into the packed weights, the bias slice of the NEXT tile is fetched during the current
+    // one (double-buffered, one barrier per tile), and the residual lands in the store staging buffer itself (every thread
+    // reads its 128-byte row into registers before it writes the same row), issued for all chunks at the start of the tile.
+    setmaxnreg_dec<kF16x3RegsEpilogue>();
+    constexpr int kCPW = BN / 32;          // 32-column chunks per warp
     const int q = warp & 3;                // 32-row quarter of the tile
-    const int half = (warp - 2) >> 2;      // which of the interleaved chunks
     const int row = q * 32 + lane;
-    const int epi_tid = (warp - 2) * 32 + lane;                              // 0 .. 255
-    uint8_t* stage_buf = smem + L::kEpiOffset + (warp - 2) * (kCPW * 4096);  // kCPW x 4 KB: residual in, result out
-    uint64_t* rbar = res_bar + (warp - 2) * 2;
+    const int epi_tid = (warp - 4) * 32 + lane;                              // 0 .. 127
+    uint8_t* stage_buf = smem + L::kEpiOffset + (warp - 4) * (kCPW * 4096);  // kCPW x 4 KB: residual in, result out
+    uint64_t* rbar = res_bar + (warp - 4) * 4;
     float* bias_s = reinterpret_cast<float*>(smem + L::kSbOffset);           // [2][BN]
     uint32_t rphase = 0;
-    WorkIter it(p, cta, grid);
+    const int cta_e = ctaid_x_here();
+    WorkIter it(p, cta_e, grid);
     int t;
     int kb0, kb1;
     uint32_t seq0 = 0;    // ring chunk number of this item's column 0
@@ -772,13 +793,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int nchunks = min(BN / 32, (p.cout - tc.n0 + 31) / 32);
       const int bsel = tile_item & 1;
       // ---- bias slices: [bsel] holds this tile's (written at the end of the previous tile, or right here for the first)
-      epi_bar_sync<256>();     // every warp is done with the tile before: its bias buffer may be refilled, this one's is visible
+      epi_bar_sync<128>();     // every warp is done with the tile before: its bias buffer may be refilled, this one's is visible
       if (tile_item == 0) {
         if (epi_tid < BN) {
           const int n = tc.n0 + epi_tid;
           bias_s[epi_tid] = (p.bias && n < p.cout) ? __ldg(p.bias + tc.batch * p.bias_z_off + n) : 0.f;
         }
-        epi_bar_sync<256>();
+        epi_bar_sync<128>();
       }
       float next_bias = 0.f;
       bool has_next = false;
@@ -799,10 +820,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (p.has_residual && lane == 0) {
 #pragma unroll
           for (int j = 0; j < kCPW; ++j) {
-            const int cj = 2 * j + half;
-            if (cj < nchunks) {
+            if (j < nchunks) {
               mbar_arrive_expect_tx(&rbar[j], 4096);
-              tma_load_4d(stage_buf + j * 4096, &tmRes, &rbar[j], tc.n0 + cj * 32 + tc.batch * p.res_c_off, box.w, box.h,
+              tma_load_4d(stage_buf + j * 4096, &tmRes, &rbar[j], tc.n0 + j * 32 + tc.batch * p.res_c_off, box.w, box.h,
                           box.res_n);
             }
           }
@@ -811,35 +831,34 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if (complete) issue_residual();
       auto load_chunk = [&](const int j, float (&acc)[32]) {
         uint32_t raw[32];
-        ring_take(ring, ring_full, ring_empty, seq0 + 2 * j + half, row, raw);
+        ring_take(ring, ring_full, ring_empty, seq0 + j, row, raw);
 #pragma unroll
         for (int i = 0; i < 32; ++i) acc[i] = __uint_as_float(raw[i]);
       };
       bool finalize = complete;
-      int c_first = cta, c_last = cta;
+      int c_first = cta_e, c_last = cta_e;
       if (!complete) {
-        // ---- publish this CTA's partial accumulator (my chunks), then find out whether it arrived last
-        float* part = sk_own_part_row(p, cta, tile_item, row, BN);
+        // ---- publish this CTA's partial accumulator (this warp's rows), then find out whether it arrived last
+        float* part = sk_own_part_row(p, cta_e, tile_item, row, BN);
 #pragma unroll
         for (int j = 0; j < kCPW; ++j) {
           uint32_t raw[32];
-          ring_take(ring, ring_full, ring_empty, seq0 + 2 * j + half, row, raw);
-          sk_publish(part, (2 * j + half) * 32, raw);
+          ring_take(ring, ring_full, ring_empty, seq0 + j, row, raw);
+          sk_publish(part, j * 32, raw);
         }
-        finalize = sk_elect_finisher<256>(p, U, grid, KB, t, epi_tid, epi_flag, c_first, c_last);
+        finalize = sk_elect_finisher<128>(p, U, grid, KB, t, epi_tid, epi_flag, c_first, c_last);
         if (finalize) issue_residual();
       }
       if (finalize) {
         const int out_n = tc.img + tc.batch * p.out_n_off;
 #pragma unroll
         for (int j = 0; j < kCPW; ++j) {
-          const int cj = 2 * j + half;
-          if (cj < nchunks) {
+          if (j < nchunks) {
             float acc[32];
             if (complete) load_chunk(j, acc);
-            else sk_reduce(p, U, grid, KB, t, c_first, c_last, row, BN, cj * 32, acc);
+            else sk_reduce(p, U, grid, KB, t, c_first, c_last, row, BN, j * 32, acc);
             uint8_t* rowp = stage_buf + j * 4096 + lane * 128;
-            const float4* biv = reinterpret_cast<const float4*>(bias_s + bsel * BN + cj * 32);
+            const float4* biv = reinterpret_cast<const float4*>(bias_s + bsel * BN + j * 32);
 #pragma unroll
             for (int i = 0; i < 32; i += 4) {
               const float4 bi = biv[i >> 2];
@@ -896,20 +915,23 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
             fence_async_smem();
             __syncwarp();
-            const int gc0 = tc.n0 + cj * 32 + tc.batch * p.out_c_off;
+            const int gc0 = tc.n0 + j * 32 + tc.batch * p.out_c_off;
             if (!OUT16 && gc0 + 32 > p.out_tail0) store_tail<false>(p, rowp, gc0, 32, box, out_n, lane);
             if (lane == 0 && gc0 < p.out_tail0) {
               tma_store_4d(&tmOut, stage_buf + j * 4096, gc0, box.w, box.h, out_n);
               tma_store_commit();
             }
           } else if (complete) {
-            ring_skip(ring, ring_full, ring_empty, seq0 + cj, row);   // columns past cout: hand the slot back unread
+            ring_skip(ring, ring_full, ring_empty, seq0 + j, row);   // columns past cout: hand the slot back unread
           }
         }
       }
       if (has_next && epi_tid < BN) bias_s[(bsel ^ 1) * BN + epi_tid] = next_bias;
     }
     if (lane == 0) tma_store_wait<0>();   // global writes complete before the CTA retires
+  } else if (PK) {
+    // warps 1..3 (barrier init done): their registers go to the MMA warpgroups
+    setmaxnreg_dec<kF16x3RegsProducer>();
   } else if (warp >= 2 && warp < 6) {
     // ===================== epilogue (warps 2..5) =====================
     const int q = warp & 3;  // 32-row quarter of the tile

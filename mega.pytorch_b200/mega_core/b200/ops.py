@@ -45,7 +45,8 @@ def _desc_flops(d):
 
 def _desc_info(d):
     return {"m": d.n_img * d.out_h * d.out_w, "batch": d.batch, "cout": d.cout, "k": d.k_per_tap,
-            "taps": d.taps_r * d.taps_s, "bn": d.block_n, "sk": d.stream_k, "res": bool(d.residual), "out16": d.out_f16}
+            "taps": d.taps_r * d.taps_s, "bn": d.block_n, "sk": d.stream_k, "res": bool(d.residual), "out16": d.out_f16,
+            "precision": d.precision}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
