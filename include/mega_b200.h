@@ -422,6 +422,15 @@ int mega_image_transform_u8(const unsigned char* src, int src_h, int src_w, long
                             long long src_pix_stride, long long src_ch_stride, const int* bounds_h, const int* kk_h, int ksize_h, const int* bounds_v, const int* kk_v, int ksize_v, int out_h,
                             int out_w, const float* mean_host, const float* std_host, int to_bgr255, float* out,
                             void* stream);
+/* mega_image_transform_u8 with an optional horizontal flip (hflip != 0): output column x takes column out_w - 1 - x
+ * of the resized image -- Resize -> RandomHorizontalFlip(1.0) -> ToTensor -> Normalize, the transform of the flipped
+ * test-time augmentation passes (reference engine/bbox_aug.py:93-101), bit-identical to PIL's FLIP_LEFT_RIGHT of the
+ * resized image. hflip == 0 is mega_image_transform_u8. */
+int mega_image_transform_u8_ex(const unsigned char* src, int src_h, int src_w, long long src_row_stride,
+                               long long src_pix_stride, long long src_ch_stride, const int* bounds_h, const int* kk_h,
+                               int ksize_h, const int* bounds_v, const int* kk_v, int ksize_v, int out_h, int out_w,
+                               const float* mean_host, const float* std_host, int to_bgr255, int hflip, float* out,
+                               void* stream);
 
 /* HOST function (no device work, all pointers are host pointers): greedy matching of one image's detections of one class,
  * already sorted by descending score, against that class's ground-truth boxes -- the inner loops of
@@ -458,6 +467,33 @@ int mega_seq_nms(const float* boxes, const float* scores, const int* labels, con
                  int max_det, const int* video_offsets, int num_videos, int num_classes, float link_iou, float nms_iou,
                  int rescore, void* workspace, long long workspace_bytes, float* out_scores, unsigned char* keep,
                  void* stream);
+
+/* ------------------------------------------------- test-time box augmentation (TEST.BBOX_AUG)
+ * Replaces the merge of the reference's im_detect_bbox_aug (engine/bbox_aug.py:11-68) for the single-frame method.
+ * Staging (the workspace): class-major [num_classes][num_passes * r_max] boxes / scores / flags; merged row
+ * pass * r_max + proposal. num_passes * r_max <= 8192; mega_bbox_aug_workspace_bytes returns -1 outside that range.
+ *
+ * mega_bbox_aug_collect: the raw post-processor output of pass `pass` (box_head/inference.py:45-86 with
+ * bbox_aug_enabled: softmax, decode with weights (wx, wy, ww, wh), clip_to_image(remove_empty=False) in the pass's
+ * im_w x im_h), then for hflip passes BoxList.transpose(FLIP_LEFT_RIGHT) in that size and BoxList.resize to the
+ * identity pass's size (engine/bbox_aug.py:15-23): x * (float)ratio_w, y * (float)ratio_h, where ratio_* = identity
+ * size / pass size as doubles (1 for the identity pass); no second clip. Rows >= *count_ptr of the pass are no
+ * candidates; a candidate scores > score_thresh. logits [r_max, ld_logits], deltas [r_max, ld_deltas] (class j at
+ * columns 4j..4j+3), proposals [r_max, 4] fp32.
+ *
+ * mega_bbox_aug_merge: filter_results over the concatenated passes (box_head/inference.py:108-149): per foreground
+ * class, NMS(nms_thresh) of the candidates in score-descending order (ties: lower merged row first), then, when more
+ * than max_det > 0 boxes survive over all classes, those scoring >= the max_det-th largest (ties kept). Output as
+ * mega_box_postprocess: class-major, merged row ascending inside a class, labels int64, *out_count = number written
+ * (<= out_cap). Reads the staging every collect of the passes 0 .. num_passes-1 wrote; alters its flags. */
+long long mega_bbox_aug_workspace_bytes(int num_passes, int r_max, int num_classes);
+int mega_bbox_aug_collect(const float* logits, int ld_logits, const float* deltas, int ld_deltas, const float* proposals,
+                          const int* count_ptr, int r_max, int num_classes, int pass, int num_passes, int im_w,
+                          int im_h, int hflip, double ratio_w, double ratio_h, float score_thresh, float wx, float wy,
+                          float ww, float wh, void* workspace, long long workspace_bytes, void* stream);
+int mega_bbox_aug_merge(int num_passes, int r_max, int num_classes, float nms_thresh, int max_det, void* workspace,
+                        long long workspace_bytes, float* out_boxes, float* out_scores, long long* out_labels,
+                        int out_cap, int* out_count, void* stream);
 
 #ifdef __cplusplus
 }

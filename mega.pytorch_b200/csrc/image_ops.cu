@@ -19,10 +19,11 @@ __global__ void image_transform_kernel(long long total, mega_image::ResizeGeom g
 
 }  // namespace mega
 
-extern "C" int mega_image_transform_u8(const unsigned char* src, int src_h, int src_w, long long src_row_stride,
-                                       long long src_pix_stride, long long src_ch_stride, const int* bounds_h, const int* kk_h, int ksize_h, const int* bounds_v,
-                                       const int* kk_v, int ksize_v, int out_h, int out_w, const float* mean_host,
-                                       const float* std_host, int to_bgr255, float* out, void* stream_v) {
+extern "C" int mega_image_transform_u8_ex(const unsigned char* src, int src_h, int src_w, long long src_row_stride,
+                                          long long src_pix_stride, long long src_ch_stride, const int* bounds_h,
+                                          const int* kk_h, int ksize_h, const int* bounds_v, const int* kk_v, int ksize_v,
+                                          int out_h, int out_w, const float* mean_host, const float* std_host,
+                                          int to_bgr255, int hflip, float* out, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   MEGA_ARG_CHECK(src_h > 0 && src_w > 0 && out_h > 0 && out_w > 0, "image_transform: empty image");
   MEGA_ARG_CHECK((src_pix_stride == 3 && src_ch_stride == 1 && src_row_stride >= 3LL * src_w) ||
@@ -43,10 +44,20 @@ extern "C" int mega_image_transform_u8(const unsigned char* src, int src_h, int 
   g.bounds_h = bounds_h, g.kk_h = kk_h, g.bounds_v = bounds_v, g.kk_v = kk_v;
   for (int c = 0; c < 3; ++c) g.mean[c] = mean_host[c], g.stdv[c] = std_host[c];
   g.to_bgr255 = to_bgr255 ? 1 : 0;
+  g.hflip = hflip ? 1 : 0;
   const long long total = static_cast<long long>(out_h) * out_w;
   long long blocks = (total + 255) / 256;
   if (blocks > 132LL * 16) blocks = 132LL * 16;
   mega::image_transform_kernel<<<static_cast<int>(blocks), 256, 0, stream>>>(total, g, src, out);
   MEGA_CUDA_CHECK(cudaGetLastError());
   return MEGA_OK;
+}
+
+extern "C" int mega_image_transform_u8(const unsigned char* src, int src_h, int src_w, long long src_row_stride,
+                                       long long src_pix_stride, long long src_ch_stride, const int* bounds_h, const int* kk_h, int ksize_h, const int* bounds_v,
+                                       const int* kk_v, int ksize_v, int out_h, int out_w, const float* mean_host,
+                                       const float* std_host, int to_bgr255, float* out, void* stream_v) {
+  return mega_image_transform_u8_ex(src, src_h, src_w, src_row_stride, src_pix_stride, src_ch_stride, bounds_h, kk_h,
+                                    ksize_h, bounds_v, kk_v, ksize_v, out_h, out_w, mean_host, std_host, to_bgr255, 0,
+                                    out, stream_v);
 }

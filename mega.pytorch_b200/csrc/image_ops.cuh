@@ -48,6 +48,7 @@ struct ResizeGeom {
   const int* kk_v;
   float mean[3], stdv[3];     // in OUTPUT channel order
   int to_bgr255;
+  int hflip = 0;              // output column x takes resized column out_w - 1 - x (FLIP_LEFT_RIGHT after Resize)
 };
 
 MEGA_IMG_HD int clip8(int v) {
@@ -79,16 +80,17 @@ MEGA_IMG_HD void horiz_rgb(const ResizeGeom& g, const uint8_t* src, int row, int
 MEGA_IMG_HD void image_transform_item(long long index, const ResizeGeom& g, const uint8_t* src, float* out) {
   const int x = static_cast<int>(index % g.out_w);
   const int y = static_cast<int>(index / g.out_w);
+  const int xs = g.hflip ? g.out_w - 1 - x : x;
   int rgb[3];
   if (g.ksize_v == 0) {
-    horiz_rgb(g, src, y, x, rgb);
+    horiz_rgb(g, src, y, xs, rgb);
   } else {
     const int ymin = g.bounds_v[2 * y], n = g.bounds_v[2 * y + 1];
     const int* k = g.kk_v + static_cast<long long>(y) * g.ksize_v;
     int s0 = 1 << (kPrecisionBits - 1), s1 = s0, s2 = s0;
     for (int j = 0; j < n; ++j) {
       int h[3];
-      horiz_rgb(g, src, ymin + j, x, h);
+      horiz_rgb(g, src, ymin + j, xs, h);
       s0 += h[0] * k[j];
       s1 += h[1] * k[j];
       s2 += h[2] * k[j];

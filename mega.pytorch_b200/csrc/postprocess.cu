@@ -7,6 +7,7 @@
 // concatenate class by class; if more than `detections_per_img` survive, keep those whose score is
 // >= the (n - D + 1)-th smallest (torch.kthvalue on the CPU, inference.py:141-148).
 #include "common.cuh"
+#include "box_head.cuh"
 #include "iou.cuh"
 #include "mega_b200.h"
 
@@ -57,31 +58,10 @@ __global__ void __launch_bounds__(kPostThreads, 1) box_class_nms_kernel(const Po
   for (int r = tid; r < p.r_max; r += blockDim.x) {
     unsigned char cand = 0;
     if (r < R) {
-      const float* l = p.logits + static_cast<long long>(r) * p.ld_logits;
-      float mx = l[0];
-      for (int c = 1; c < p.num_classes; ++c) mx = fmaxf(mx, l[c]);
-      float sum = 0.f;
-      for (int c = 0; c < p.num_classes; ++c) sum = __fadd_rn(sum, expf(__fsub_rn(l[c], mx)));
-      const float prob = __fdiv_rn(expf(__fsub_rn(l[j], mx)), sum);
-      const float* d = p.deltas + static_cast<long long>(r) * p.ld_deltas + j * 4;
+      const float prob = class_softmax_prob(p.logits + static_cast<long long>(r) * p.ld_logits, p.num_classes, j);
       const float4 box = *reinterpret_cast<const float4*>(p.proposals + static_cast<long long>(r) * 4);
-      // BoxCoder.decode (box_coder.py:52-95)
-      const float widths = __fadd_rn(__fsub_rn(box.z, box.x), 1.f), heights = __fadd_rn(__fsub_rn(box.w, box.y), 1.f);
-      const float ctr_x = __fadd_rn(box.x, __fmul_rn(0.5f, widths)), ctr_y = __fadd_rn(box.y, __fmul_rn(0.5f, heights));
-      const float clipv = 4.135166556742356f;
-      const float dx = __fdiv_rn(d[0], p.wx), dy = __fdiv_rn(d[1], p.wy);
-      const float dw = fminf(__fdiv_rn(d[2], p.ww), clipv), dh = fminf(__fdiv_rn(d[3], p.wh), clipv);
-      const float pcx = __fadd_rn(__fmul_rn(dx, widths), ctr_x), pcy = __fadd_rn(__fmul_rn(dy, heights), ctr_y);
-      const float pw = __fmul_rn(expf(dw), widths), ph = __fmul_rn(expf(dh), heights);
-      float4 o;
-      o.x = __fsub_rn(pcx, __fmul_rn(0.5f, pw));
-      o.y = __fsub_rn(pcy, __fmul_rn(0.5f, ph));
-      o.z = __fsub_rn(__fadd_rn(pcx, __fmul_rn(0.5f, pw)), 1.f);
-      o.w = __fsub_rn(__fadd_rn(pcy, __fmul_rn(0.5f, ph)), 1.f);
-      o.x = fminf(fmaxf(o.x, 0.f), p.im_w - 1.f);
-      o.y = fminf(fmaxf(o.y, 0.f), p.im_h - 1.f);
-      o.z = fminf(fmaxf(o.z, 0.f), p.im_w - 1.f);
-      o.w = fminf(fmaxf(o.w, 0.f), p.im_h - 1.f);
+      const float4 o = decode_clip_box(p.deltas + static_cast<long long>(r) * p.ld_deltas + j * 4, box,
+                                       BoxCoderW{p.wx, p.wy, p.ww, p.wh}, p.im_w, p.im_h);
       ob[r] = o;
       os[r] = prob;
       cand = prob > p.score_thresh;
@@ -146,17 +126,6 @@ __global__ void __launch_bounds__(kPostThreads, 1) box_class_nms_kernel(const Po
     }
   }
 }
-
-struct FinalParams {
-  const float4* cls_boxes;
-  const float* cls_scores;
-  const unsigned char* cls_keep;
-  int r_max, num_classes, max_det, out_cap;
-  float* out_boxes;        // [out_cap,4]
-  float* out_scores;       // [out_cap]
-  long long* out_labels;   // [out_cap]
-  int* out_count;
-};
 
 __global__ void __launch_bounds__(1024, 1) box_final_kernel(const FinalParams p) {
   __shared__ int hist[256];
@@ -248,6 +217,8 @@ __global__ void __launch_bounds__(1024, 1) box_final_kernel(const FinalParams p)
   if (tid == 0) p.out_count[0] = min(s_running, p.out_cap);
 }
 
+void launch_box_final(const FinalParams& f, cudaStream_t stream) { box_final_kernel<<<1, 1024, 0, stream>>>(f); }
+
 static size_t align_up_pp(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 }  // namespace mega
@@ -309,7 +280,7 @@ extern "C" int mega_box_postprocess(const float* logits, int ld_logits, const fl
   f.out_scores = out_scores;
   f.out_labels = out_labels;
   f.out_count = out_count;
-  box_final_kernel<<<1, 1024, 0, stream>>>(f);
+  launch_box_final(f, stream);
   MEGA_CUDA_CHECK(cudaGetLastError());
   return MEGA_OK;
 }

@@ -569,6 +569,11 @@ class MlpHeadMixin:
 
     def _mlp_head(self, feats, im_w, im_h):
         """feats [1, h, w, 1024] (backbone map, or its aggregated / warped replacement) -> Detections"""
+        f7, boxes, cnt = self._mlp_features(feats, im_w, im_h)
+        return self.predict_and_postprocess(f7, boxes, cnt, im_w, im_h)
+
+    def _mlp_features(self, feats, im_w, im_h):
+        """RPN -> res5 -> ROIAlign -> fc6 -> fc7: (fc7 rows, proposals [KP, 4], device count [1])"""
         c = self.cfg
         KP = c.post_nms_top_n
         boxes, _, cnt = self.rpn(feats, im_w, im_h, KP)
@@ -582,7 +587,7 @@ class MlpHeadMixin:
         f7 = self._buf("fc7", (KP, self.fc7_w.shape[0]), self.act)
         ops.linear(f6, self.fc7_w, f7, bias=self.fc7_b, relu=True)
         self.last_feats, self.last_props, self.last_cnt, self.last_pooled = feats, boxes[0], cnt, pooled
-        return self.predict_and_postprocess(f7, boxes[0], cnt[0:1], im_w, im_h)
+        return f7, boxes[0], cnt[0:1]
 
 
 class WindowedEngine(HeadCommon):
@@ -1521,6 +1526,36 @@ class BaseEngine(HeadCommon, MlpHeadMixin):
     @_with_precision
     def forward(self, img, im_w, im_h):
         return self._mlp_head(self.backbone.forward(img), im_w, im_h)
+
+    @_with_precision
+    def forward_bbox_aug(self, passes, num_passes, im_w, im_h, trace=None):
+        """test-time box augmentation of one image (engine/bbox_aug.py:11-68) -> Detections in the im_w x im_h frame of
+        the identity pass. passes: iterable of num_passes (img [1, 3, h, w], w, h, hflip), the identity pass first, in
+        the reference's order (mega_core.engine.bbox_aug.aug_plan); consumed one at a time. Each pass runs the whole
+        detector up to the predictor GEMM, and a collect launch stages its raw post-processor output, mapped to the
+        identity frame, in slot `pass` of a class-major staging area; one merge launch pair then applies filter_results to
+        all passes. Stream order lets each pass reuse the proposal and predictor buffers once the previous collect ran.
+        trace: a list that gets (proposals, count, predictor rows) copies of every pass."""
+        c = self.cfg
+        kp, ncls = c.post_nms_top_n, self.num_classes
+        ws = self._buf("aug_ws", (ops.bbox_aug_workspace_bytes(num_passes, kp, ncls),), torch.uint8)
+        a = -1
+        for a, (img, w, h, hflip) in enumerate(passes):
+            if a >= num_passes:
+                raise ValueError("forward_bbox_aug: more than num_passes=%d passes" % num_passes)
+            f7, boxes, cnt = self._mlp_features(self.backbone.forward(img), w, h)
+            pred = self.predict_gemm(f7)
+            ops.bbox_aug_collect(pred[:, :ncls], pred[:, ncls:], boxes, cnt, ncls, a, num_passes, w, h, hflip,
+                                 float(im_w) / float(w), float(im_h) / float(h), c.score_thresh, c.bbox_reg_weights, ws)
+            if trace is not None:
+                trace.append((boxes.clone(), cnt.clone(), pred.clone()))
+        if a != num_passes - 1:
+            raise ValueError("forward_bbox_aug: got %d passes, expected %d" % (a + 1, num_passes))
+        cap = (ncls - 1) * num_passes * kp
+        out = (self._buf("aug_boxes", (cap, 4)), self._buf("aug_scores", (cap,)),
+               self._buf("aug_labels", (cap,), torch.int64), self._buf("aug_count", (1,), torch.int32))
+        ops.bbox_aug_merge(num_passes, kp, ncls, c.nms_thresh, c.detections_per_img, ws, out)
+        return Detections(*out)
 
 
 # =============================================================================================== FGFA (SURVEY row a19)

@@ -953,6 +953,42 @@ def box_postprocess(logits, deltas, proposals, count, num_classes, im_w, im_h, s
     return out
 
 
+def bbox_aug_workspace_bytes(num_passes, r_max, num_classes):
+    """bytes of the class-major staging area of test-time box augmentation (csrc/bbox_aug.cu)"""
+    nbytes = lib.mega_bbox_aug_workspace_bytes(num_passes, r_max, num_classes)
+    if nbytes < 0:
+        raise _lib.MegaError("bbox_aug: %d passes x %d proposals = %d merged rows per class, %d classes: out of range "
+                             "(at most 8192 merged rows, at least 2 classes)"
+                             % (num_passes, r_max, num_passes * r_max, num_classes))
+    return nbytes
+
+
+def bbox_aug_collect(logits, deltas, proposals, count, num_classes, pass_index, num_passes, im_w, im_h, hflip, ratio_w,
+                     ratio_h, score_thresh, weights, workspace):
+    """stage one pass's raw detections, mapped to the identity frame, in slot `pass_index` of `workspace` (uint8).
+    logits / deltas: [R, ld] views (may alias one buffer); proposals [R, 4]; count: device int32 [1]; ratio_*: Python
+    floats identity size / pass size"""
+    require_cuda(logits, deltas, proposals, count, workspace)
+    r = proposals.shape[0]
+    check(lib.mega_bbox_aug_collect(ptr(logits), logits.stride(0), ptr(deltas), deltas.stride(0), ptr(proposals),
+                                    ptr(count), r, num_classes, pass_index, num_passes, int(im_w), int(im_h),
+                                    int(bool(hflip)), float(ratio_w), float(ratio_h), float(score_thresh),
+                                    *[float(x) for x in weights], ptr(workspace), workspace.numel(), stream_ptr()),
+          "mega_bbox_aug_collect")
+    LAUNCHES[0] += 1
+
+
+def bbox_aug_merge(num_passes, r_max, num_classes, nms_thresh, max_det, workspace, out):
+    """filter_results over the staged passes; out = (boxes, scores, labels int64, count int32 [1])"""
+    require_cuda(workspace, *out)
+    ob, os_, ol, oc = out
+    check(lib.mega_bbox_aug_merge(num_passes, r_max, num_classes, float(nms_thresh), int(max_det), ptr(workspace),
+                                  workspace.numel(), ptr(ob), ptr(os_), ptr(ol), ob.shape[0], ptr(oc), stream_ptr()),
+          "mega_bbox_aug_merge")
+    LAUNCHES[0] += 2
+    return out
+
+
 SEQ_NMS_RESCORE = {"avg": 0, "max": 1}
 
 

@@ -37,6 +37,24 @@ def synthetic_frame(index, height=600, width=1000, seed=1000, boxes=4):
     return img.unsqueeze(0).contiguous()
 
 
+def synthetic_image_u8(height, width, seed=5, blobs=12):
+    """uint8 [H, W, 3] RGB image, as a decoder would hand it to the input transform: flat-coloured discs on a black
+    background plus uniform noise in [-20, 20]. Integer arithmetic only, so every machine regenerates the same bytes."""
+    g = torch.Generator().manual_seed(seed)
+    yy = torch.arange(height).view(-1, 1)
+    xx = torch.arange(width).view(1, -1)
+    img = torch.zeros(height, width, 3, dtype=torch.int64)
+    for _ in range(blobs):
+        cy = int(torch.randint(0, height, (1,), generator=g))
+        cx = int(torch.randint(0, width, (1,), generator=g))
+        r = int(torch.randint(10, 60, (1,), generator=g))
+        col = torch.randint(0, 256, (3,), generator=g)
+        m = ((yy - cy) ** 2 + (xx - cx) ** 2) < r * r
+        img[m] = col
+    img = img + torch.randint(-20, 21, (height, width, 3), generator=g)
+    return img.clamp(0, 255).to(torch.uint8)
+
+
 def _kaiming(shape, gen, gain=math.sqrt(2.0)):
     fan_in = 1
     for d in shape[1:]:

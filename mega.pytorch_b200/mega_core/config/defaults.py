@@ -140,7 +140,9 @@ _C = CfgNode({
     "SOLVER": {"BASE_LR": 0.001, "WEIGHT_DECAY": 0.0005, "STEPS": (30000,), "MAX_ITER": 40000, "IMS_PER_BATCH": 16,
                "WARMUP_ITERS": 500},
     "TEST": {"EXPECTED_RESULTS": [], "EXPECTED_RESULTS_SIGMA_TOL": 4, "IMS_PER_BATCH": 8, "DETECTIONS_PER_IMG": 100,
-             "BBOX_AUG": {"ENABLED": False}},
+             # test-time box augmentation (config/defaults.py:511-526), single-frame method only
+             # (mega_core.engine.bbox_aug)
+             "BBOX_AUG": {"ENABLED": False, "H_FLIP": False, "SCALES": (), "MAX_SIZE": 4000, "SCALE_H_FLIP": False}},
     "OUTPUT_DIR": ".", "DTYPE": "float32", "AMP_VERBOSE": False,
     "PATHS_CATALOG": os.path.join(os.path.dirname(os.path.abspath(__file__)), "paths_catalog.py"),
 })

@@ -3,7 +3,7 @@ GPU for the video methods, whole videos per rank when distributed."""
 import torch.utils.data
 
 from . import datasets as D
-from .collate_batch import BatchCollator
+from .collate_batch import BatchCollator, BBoxAugCollator
 from .samplers import VIDTestDistributedSampler
 from .transforms import build_transforms
 from ..utils.comm import get_world_size
@@ -33,8 +33,12 @@ def make_data_loader(cfg, is_train=False, is_distributed=False, start_iter=0, is
     if dataset_catalog is None:
         from ..config.paths_catalog import DatasetCatalog as dataset_catalog
     method = cfg.MODEL.VID.METHOD
-    device_side = transforms is None
-    if device_side:
+    # TEST.BBOX_AUG.ENABLED (data/build.py:165, :175-176): no dataset transform, im_detect_bbox_aug transforms each pass
+    bbox_aug = cfg.TEST.BBOX_AUG.ENABLED
+    device_side = transforms is None and not bbox_aug
+    if bbox_aug:
+        transforms = None
+    elif device_side:
         transforms = build_transforms(cfg, is_train=False)
     loaders = []
     for dataset in build_dataset(cfg.DATASETS.TEST, transforms, dataset_catalog, False, method):
@@ -52,6 +56,7 @@ def make_data_loader(cfg, is_train=False, is_distributed=False, start_iter=0, is
             sampler = torch.utils.data.sampler.SequentialSampler(dataset)
         batches = torch.utils.data.sampler.BatchSampler(sampler, per_batch // world, drop_last=False)
         loaders.append(torch.utils.data.DataLoader(
-            dataset, batch_sampler=batches, collate_fn=BatchCollator(cfg.DATALOADER.SIZE_DIVISIBILITY, method, False),
+            dataset, batch_sampler=batches,
+            collate_fn=BBoxAugCollator() if bbox_aug else BatchCollator(cfg.DATALOADER.SIZE_DIVISIBILITY, method, False),
             num_workers=0 if device_side else cfg.DATALOADER.NUM_WORKERS))   # CUDA tensors cannot cross worker processes
     return loaders

@@ -26,3 +26,11 @@ class BatchCollator(object):
             else:
                 images[key] = value
         return images, targets, ids
+
+
+class BBoxAugCollator(object):
+    """data/collate_batch.py:42-50: with TEST.BBOX_AUG.ENABLED the dataset yields untransformed images; the batch stays
+    (images, targets, image ids) tuples and mega_core.engine.bbox_aug.im_detect_bbox_aug transforms every image itself"""
+
+    def __call__(self, batch):
+        return list(zip(*batch))

@@ -82,7 +82,7 @@ class DeviceTestTransform(object):
     tensor (what `decode_jpeg` below / torchvision.io.decode_jpeg(device="cuda") returns: nvJPEG output is consumed in
     place, no re-layout). Returns a float32 [3, H', W'] device tensor."""
 
-    def __init__(self, min_size, max_size, mean, std, to_bgr255=True, device="cuda"):
+    def __init__(self, min_size, max_size, mean, std, to_bgr255=True, device="cuda", hflip=False):
         if isinstance(min_size, (list, tuple)):
             assert len(min_size) == 1, "test-time transform: a single MIN_SIZE_TEST"
             min_size = min_size[0]
@@ -90,6 +90,7 @@ class DeviceTestTransform(object):
         self.mean = np.asarray(mean, dtype=np.float32)
         self.std = np.asarray(std, dtype=np.float32)
         self.to_bgr255 = bool(to_bgr255)
+        self.hflip = bool(hflip)          # RandomHorizontalFlip(1.0) after Resize: the flipped test-time augmentation passes
         self.device = torch.device(device)
         self._tables = {}
 
@@ -127,13 +128,17 @@ class DeviceTestTransform(object):
         if out is None:
             out = torch.empty(3, oh, ow, device=self.device)
         assert out.shape == (3, oh, ow) and out.dtype == torch.float32 and out.is_contiguous()
-        _lib.check(_lib.lib.mega_image_transform_u8(
-            _lib.ptr(src), h, w, row, pix, ch, _lib.ptr(bh), _lib.ptr(kh), ksh, _lib.ptr(bv), _lib.ptr(kv), ksv, oh, ow,
-            self.mean.ctypes.data, self.std.ctypes.data, int(self.to_bgr255), _lib.ptr(out), _lib.stream_ptr()),
-            "mega_image_transform_u8")
+        args = (_lib.ptr(src), h, w, row, pix, ch, _lib.ptr(bh), _lib.ptr(kh), ksh, _lib.ptr(bv), _lib.ptr(kv), ksv, oh,
+                ow, self.mean.ctypes.data, self.std.ctypes.data, int(self.to_bgr255))
+        if self.hflip:
+            _lib.check(_lib.lib.mega_image_transform_u8_ex(*args, 1, _lib.ptr(out), _lib.stream_ptr()),
+                       "mega_image_transform_u8_ex")
+        else:
+            _lib.check(_lib.lib.mega_image_transform_u8(*args, _lib.ptr(out), _lib.stream_ptr()), "mega_image_transform_u8")
         if target is not None and hasattr(target, "resize"):
             target = target.resize((ow, oh))
         return out, target
 
     def __repr__(self):
-        return "DeviceTestTransform(min_size=%s, max_size=%s, to_bgr255=%s)" % (self.min_size, self.max_size, self.to_bgr255)
+        return "DeviceTestTransform(min_size=%s, max_size=%s, to_bgr255=%s, hflip=%s)" % (
+            self.min_size, self.max_size, self.to_bgr255, self.hflip)

@@ -13,6 +13,7 @@ import torch
 
 from ..data.datasets.evaluation.vid import vid_evaluation
 from ..utils.comm import gather_predictions, get_world_size, is_main_process, synchronize
+from .bbox_aug import im_detect_bbox_aug
 from .seq_nms import seq_nms_predictions
 
 
@@ -46,9 +47,11 @@ def _to_device(images, device, method):
 
 
 def compute_on_dataset(model, data_loader, device, bbox_aug, method, timer=None):
-    """engine/inference.py:18-47 -> {image_id: BoxList on the CPU}"""
-    if bbox_aug:
-        raise NotImplementedError("test-time box augmentation is not part of the B200 build")
+    """engine/inference.py:18-47 -> {image_id: BoxList on the CPU}. bbox_aug: TEST.BBOX_AUG.ENABLED, the batches are
+    BBoxAugCollator's (untransformed images) and im_detect_bbox_aug runs them; single-frame method only"""
+    if bbox_aug and method != "base":
+        raise NotImplementedError("TEST.BBOX_AUG.ENABLED: test-time box augmentation is defined for MODEL.VID.METHOD "
+                                  "'base' only, not for '%s'" % method)
     model.eval()
     results = {}
     cpu = torch.device("cpu")
@@ -56,7 +59,10 @@ def compute_on_dataset(model, data_loader, device, bbox_aug, method, timer=None)
         with torch.no_grad():
             if timer:
                 timer.tic()
-            output = model(_to_device(images, device, method))
+            if bbox_aug:
+                output = im_detect_bbox_aug(model, images, device)
+            else:
+                output = model(_to_device(images, device, method))
             if timer:
                 if device.type != "cpu":
                     torch.cuda.synchronize()
