@@ -495,6 +495,28 @@ int mega_bbox_aug_merge(int num_passes, int r_max, int num_classes, float nms_th
                         long long workspace_bytes, float* out_boxes, float* out_scores, long long* out_labels,
                         int out_cap, int* out_count, void* stream);
 
+/* ------------------------------------------------------- proposal recall (box_only evaluation)
+ * eval_proposals_vid of the reference (data/datasets/evaluation/vid/vid_eval.py:72-119) for a whole dataset in one launch.
+ * Input, flattened per image i in [0, num_images) (device memory): proposals [prop_offsets[i], prop_offsets[i+1]) of
+ * prop_boxes [sum P, 4] xyxy fp32 (16-byte aligned) with prop_scores (objectness), ground truth [gt_offsets[i],
+ * gt_offsets[i+1]) of gt_boxes [sum G, 4]. max_props >= every P (at most 8192), max_gt >= every G. Per image:
+ *   1. the proposals ordered by objectness, descending (ties: lower index first), the first `limit` kept (P');
+ *   2. the P' x G IoU matrix, boxlist_iou's "+1" arithmetic, every fp32 operation rounded separately;
+ *   3. min(P', G) rounds: the largest entry (ties: lower GT index, then lower proposal index) is written to
+ *      gt_overlaps[gt_offsets[i] + round], its row and column are set to -1; gt_overlaps of the image past min(P', G),
+ *      and of images with P' = 0 or G = 0, are 0.
+ * stats (3 x uint64, device memory, zeroed by the call): [0] the overlaps >= iou_thresh of the images with P' > 0 and
+ * G > 0 (all G entries of each), [1] num_pos = sum of G over all images, [2] images whose P or G exceeds max_props /
+ * max_gt (skipped; their GT still counts in num_pos; a correct call gives 0). Recall = stats[0] / stats[1].
+ * Deterministic. workspace: >= mega_proposal_recall_workspace_bytes(num_images, max_props, max_gt, limit) bytes, 256-byte
+ * aligned (0 bytes, workspace may be null, while min(max_props, limit) x max_gt x 4 <= 32 KB); returns -1 for arguments
+ * out of range. */
+long long mega_proposal_recall_workspace_bytes(int num_images, int max_props, int max_gt, int limit);
+int mega_proposal_recall(const float* prop_boxes, const float* prop_scores, const long long* prop_offsets,
+                         const float* gt_boxes, const long long* gt_offsets, int num_images, int max_props, int max_gt,
+                         int limit, float iou_thresh, void* workspace, long long workspace_bytes, float* gt_overlaps,
+                         unsigned long long* stats, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -238,6 +238,10 @@ lib.mega_bbox_aug_collect.argtypes = [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _i, _i
 lib.mega_bbox_aug_collect.restype = _i
 lib.mega_bbox_aug_merge.argtypes = [_i, _i, _i, _f, _i, _vp, _ll, _vp, _vp, _vp, _i, _vp, _vp]
 lib.mega_bbox_aug_merge.restype = _i
+lib.mega_proposal_recall_workspace_bytes.argtypes = [_i, _i, _i, _i]
+lib.mega_proposal_recall_workspace_bytes.restype = _ll
+lib.mega_proposal_recall.argtypes = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _ll, _vp, _vp, _vp]
+lib.mega_proposal_recall.restype = _i
 
 EXPORTS = [
     "mega_last_error", "mega_abi_version", "mega_device_ok", "mega_conv_gemm", "mega_conv_gemm_tf32", "mega_conv_gemm_workspace_bytes", "mega_set_tf32_rounding",
@@ -255,4 +259,5 @@ EXPORTS = [
     "mega_image_transform_u8", "mega_dff_warp_scale", "mega_vid_match_host", "mega_split16_pack", "mega_split16_unpack", "mega_relation_softmax_split16", "mega_relation_softmax_pe_split16", "mega_roi_align_forward_nhwc_split16",
     "mega_seq_nms_workspace_bytes", "mega_seq_nms",
     "mega_image_transform_u8_ex", "mega_bbox_aug_workspace_bytes", "mega_bbox_aug_collect", "mega_bbox_aug_merge",
+    "mega_proposal_recall_workspace_bytes", "mega_proposal_recall",
 ]

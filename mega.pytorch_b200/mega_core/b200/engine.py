@@ -66,6 +66,9 @@ class EngineConfig:
     #   "tf32"   fp32 tensors, operands rounded to TF32 by the TMA load
     #   "fp32x3" fp32 tensors, 3xTF32 split: near-fp32 contractions, the strict-parity mode
     precision = "tf32"
+    # MODEL.RPN_ONLY (single-frame, DFF and FGFA engines): the result is the RPN's proposals; the box head (res5, the
+    # channel reduction, ROIAlign, fc6 / fc7, the predictor) is neither loaded nor run
+    rpn_only = False
 
     def __init__(self, **kw):
         for k, v in kw.items():
@@ -368,11 +371,26 @@ class Detections:
         return self.boxes[:n].cpu(), self.scores[:n].cpu(), self.labels[:n].cpu()
 
 
+class Proposals:
+    """device-side RPN-only result of one frame (MODEL.RPN_ONLY): padded buffers + count, rows in descending objectness
+    order (mega_rpn_select keeps its sorted order through NMS)"""
+
+    def __init__(self, boxes, objectness, count):
+        self.boxes, self.objectness, self.count = boxes, objectness, count
+
+    def to_host(self):
+        n = int(self.count.item())
+        return self.boxes[:n].cpu(), self.objectness[:n].cpu()
+
+
 class HeadCommon:
     """pieces shared by the MEGA and single-frame engines: RPN head + selection, res5, predictor."""
 
     def __init__(self, sd, cfg, dev):
         self.cfg, self.dev = cfg, dev
+        if cfg.rpn_only and not isinstance(self, MlpHeadMixin):
+            raise NotImplementedError("MODEL.RPN_ONLY: served by the single-frame, DFF and FGFA engines only, not by %s"
+                                      % type(self).__name__)
         # per-shape (tile width, scheduling) selection by on-device timing the first time a shape is seen
         ops.AUTOTUNE[0] = os.environ.get("MEGA_B200_AUTOTUNE", "1") != "0"
         ops.load_tuned(os.environ.get("MEGA_B200_TUNED", os.path.join(os.path.dirname(__file__), "tuned_b200.json")))
@@ -390,6 +408,15 @@ class HeadCommon:
         self.rpn_ld = _round_up(5 * a, 4)
         self.base_anchors = cell_anchors(cfg.anchor_stride, cfg.anchor_sizes, cfg.aspect_ratios).to(dev)
         assert self.base_anchors.shape[0] == a
+        self._bufs = {}
+        self._chains = {}
+        self.chained = self.act == torch.float16          # fp16 mode: conv chains run as persistent multi-layer kernels
+        self.reduce = False
+        if not cfg.rpn_only:
+            self._init_box_head(sd)
+
+    def _init_box_head(self, sd):
+        dev, act, cfg = self.dev, self.act, self.cfg
         self.res5 = ResNetStages(sd, FE + "head.", (4,), dev, dilation=cfg.res5_dilation,
                                  first_stride_of=lambda li: 1, dtype=act)
         self.reduce = (FE + "conv.weight") in sd          # REDUCE_CHANNEL: 1x1 conv 2048 -> 256 + ReLU after res5
@@ -405,9 +432,6 @@ class HeadCommon:
         pb[:5 * self.num_classes] = torch.cat([sd["roi_heads.box.predictor.cls_score.bias"].float(),
                                                sd["roi_heads.box.predictor.bbox_pred.bias"].float()])
         self.pred_b = pb.contiguous().to(dev)
-        self._bufs = {}
-        self._chains = {}
-        self.chained = self.act == torch.float16          # fp16 mode: conv chains run as persistent multi-layer kernels
 
     def _buf(self, tag, shape, dtype=torch.float32):
         key = (tag, tuple(shape), dtype)
@@ -555,6 +579,8 @@ class MlpHeadMixin:
     ROIAlign -> fc6 -> fc7 -> predictor -> post-processing (ResNetConv52MLPFeatureExtractor, extractors :106-118)"""
 
     def _init_mlp_head(self, sd):
+        if self.cfg.rpn_only:
+            return
         dev, act = self.dev, self.act
         res = self.cfg.pooler_resolution
         w6 = sd[FE + "fc6.weight"].float()
@@ -566,6 +592,20 @@ class MlpHeadMixin:
         self.fc6_b = sd[FE + "fc6.bias"].float().contiguous().to(dev)
         self.fc7_w = sd[FE + "fc7.weight"].float().contiguous().to(dev).to(act)
         self.fc7_b = sd[FE + "fc7.bias"].float().contiguous().to(dev)
+
+    def _head(self, feats, im_w, im_h):
+        """feats [1, h, w, 1024] (backbone map, or its aggregated / warped replacement) -> Detections, or under
+        cfg.rpn_only the proposals the box head would have received"""
+        if self.cfg.rpn_only:
+            return self._proposals(feats, im_w, im_h)
+        return self._mlp_head(feats, im_w, im_h)
+
+    def _proposals(self, feats, im_w, im_h):
+        """RPN only (RPNModule._forward_test with an empty roi_heads, rpn/rpn.py:186-197): POST_NMS_TOP_N_TEST proposals,
+        already in descending objectness order, so the reference's sort needs no launch"""
+        boxes, scores, cnt = self.rpn(feats, im_w, im_h, self.cfg.post_nms_top_n)
+        self.last_feats, self.last_props, self.last_cnt = feats, boxes[0], cnt
+        return Proposals(boxes[0], scores[0], cnt[0:1])
 
     def _mlp_head(self, feats, im_w, im_h):
         """feats [1, h, w, 1024] (backbone map, or its aggregated / warped replacement) -> Detections"""
@@ -1525,7 +1565,7 @@ class BaseEngine(HeadCommon, MlpHeadMixin):
 
     @_with_precision
     def forward(self, img, im_w, im_h):
-        return self._mlp_head(self.backbone.forward(img), im_w, im_h)
+        return self._head(self.backbone.forward(img), im_w, im_h)
 
     @_with_precision
     def forward_bbox_aug(self, passes, num_passes, im_w, im_h, trace=None):
@@ -1537,6 +1577,9 @@ class BaseEngine(HeadCommon, MlpHeadMixin):
         all passes. Stream order lets each pass reuse the proposal and predictor buffers once the previous collect ran.
         trace: a list that gets (proposals, count, predictor rows) copies of every pass."""
         c = self.cfg
+        if c.rpn_only:
+            raise NotImplementedError("MODEL.RPN_ONLY with TEST.BBOX_AUG.ENABLED: test-time augmentation merges class "
+                                      "detections, which an RPN-only model does not produce")
         kp, ncls = c.post_nms_top_n, self.num_classes
         ws = self._buf("aug_ws", (ops.bbox_aug_workspace_bytes(num_passes, kp, ncls),), torch.uint8)
         a = -1
@@ -1805,7 +1848,7 @@ class FgfaEngine(HeadCommon, MlpHeadMixin):
         flow = self.flownet.forward(self.pairs)
         self.last_flow = flow
         ops.fgfa_aggregate(self.ring, self.slots_d, self.KL, flow, self.agg[0], 1024, 2048)
-        return self._mlp_head(self.agg, im_w, im_h)
+        return self._head(self.agg, im_w, im_h)
 
 
 # =============================================================================================== DFF (SURVEY 8f row 4)
@@ -1863,4 +1906,4 @@ class DffEngine(HeadCommon, MlpHeadMixin):
         flow, scale = self.flownet.forward(self.pairs[1:2], want_scale=True)
         self.last_flow, self.last_scale = flow, scale
         ops.dff_warp_scale(self.key_feats[0], flow[0], scale[0], self.warped[0])
-        return self._mlp_head(self.warped, im_w, im_h)
+        return self._head(self.warped, im_w, im_h)

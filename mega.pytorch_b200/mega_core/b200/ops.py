@@ -1025,6 +1025,31 @@ def seq_nms(boxes, scores, labels, counts, video_offsets, num_classes, link_iou=
     return out_scores, keep
 
 
+def proposal_recall_workspace_bytes(num_images, max_props, max_gt, limit):
+    nbytes = lib.mega_proposal_recall_workspace_bytes(num_images, max_props, max_gt, limit)
+    if nbytes < 0:
+        raise _lib.MegaError("proposal_recall: %d images of at most %d proposals and %d GT boxes, limit %d: out of range "
+                             "(at most 8192 proposals per image)" % (num_images, max_props, max_gt, limit))
+    return nbytes
+
+
+def proposal_recall(prop_boxes, prop_scores, prop_offsets, gt_boxes, gt_offsets, max_props, max_gt, limit, iou_thresh,
+                    gt_overlaps, stats):
+    """eval_proposals_vid over many images in one launch (include/mega_b200.h, mega_proposal_recall). prop_boxes [P, 4]
+    fp32, prop_scores [P], gt_boxes [G, 4], prop_offsets / gt_offsets [N + 1] int64; outputs gt_overlaps [G] fp32 and
+    stats [3] int64 (hits, num_pos, images over max_props / max_gt). The workspace, when the IoU matrices outgrow shared
+    memory, is allocated for this call only. No synchronisation."""
+    require_cuda(prop_boxes, prop_scores, prop_offsets, gt_boxes, gt_offsets, gt_overlaps, stats)
+    n = prop_offsets.numel() - 1
+    nbytes = proposal_recall_workspace_bytes(n, max_props, max_gt, limit)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=stats.device) if nbytes else None
+    check(lib.mega_proposal_recall(ptr(prop_boxes), ptr(prop_scores), ptr(prop_offsets), ptr(gt_boxes), ptr(gt_offsets), n,
+                                   int(max_props), int(max_gt), int(limit), float(iou_thresh), ptr(ws), nbytes,
+                                   ptr(gt_overlaps), ptr(stats), stream_ptr()),
+          "mega_proposal_recall")
+    LAUNCHES[0] += 1
+
+
 # --------------------------------------------------------------------------- FGFA helpers (csrc/fgfa.cu)
 def _is16(t):
     return 1 if t.dtype == torch.float16 else 0

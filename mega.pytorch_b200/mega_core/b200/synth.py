@@ -10,6 +10,7 @@ the 690 MB of weights are never stored).
 """
 import math
 
+import numpy as np
 import torch
 
 PIXEL_MEAN = (102.9801, 115.9465, 122.7717)  # config/defaults.py:51-55 (BGR, 0-255 domain)
@@ -217,3 +218,31 @@ def global_frame_indices(seg_len, size=10, seed=0):
     a seeded torch permutation here -- only determinism matters for synthetic video)."""
     g = torch.Generator().manual_seed(seed)
     return torch.randperm(seg_len, generator=g).tolist()
+
+
+def synthetic_proposal_dataset(seed=0, num_images=176126, max_props=300, max_gt=4, tail_images=64, tail_props=1000,
+                               tail_gt=200):
+    """a seeded proposal-recall workload the size of ImageNet-VID val (176,126 frames): per image 0..max_props proposals
+    (objectness rounded to 3 decimals, so ties occur) and 0..max_gt GT boxes on integer pixels of a 1000 x 600 frame,
+    then `tail_images` images with up to `tail_props` proposals and `tail_gt` GT boxes. Packed flat:
+    (prop_boxes [P, 4] fp32, objectness [P], gt_boxes [G, 4], prop_offsets [N + 1] int64, gt_offsets [N + 1] int64)"""
+    g = np.random.default_rng(seed)
+    n_p = np.concatenate([g.integers(0, max_props + 1, num_images), g.integers(tail_props // 2, tail_props + 1, tail_images)])
+    n_g = np.concatenate([g.integers(0, max_gt + 1, num_images), g.integers(tail_gt // 2, tail_gt + 1, tail_images)])
+
+    def boxes(n):
+        xy = g.integers(0, 900, (n, 2)).astype(np.float32)
+        return np.concatenate([xy, xy + g.integers(8, 200, (n, 2)).astype(np.float32)], 1)
+
+    po = np.concatenate([[0], np.cumsum(n_p)]).astype(np.int64)
+    go = np.concatenate([[0], np.cumsum(n_g)]).astype(np.int64)
+    pb = boxes(int(po[-1]))
+    gb = boxes(int(go[-1]))
+    # a third of the proposals sit near a GT box of their image, so the recall is not trivially 0
+    img = np.repeat(np.arange(len(n_p)), n_p)
+    has = n_g[img] > 0
+    pick = has & (g.random(len(img)) < 1 / 3)
+    gsel = go[img[pick]] + (g.random(int(pick.sum())) * n_g[img[pick]]).astype(np.int64)
+    pb[pick] = gb[gsel] + g.integers(-6, 7, (int(pick.sum()), 4)).astype(np.float32)
+    scores = np.round(g.random(len(img)), 3).astype(np.float32)
+    return pb, scores, gb, po, go

@@ -1,5 +1,5 @@
 from .vid_eval import (calc_detection_vid_ap, calc_detection_vid_prec_rec, do_vid_evaluation,  # noqa: F401
-                       eval_detection_vid)
+                       eval_detection_vid, eval_proposals_vid)
 
 
 def vid_evaluation(dataset, predictions, output_folder, box_only, motion_specific, **_):

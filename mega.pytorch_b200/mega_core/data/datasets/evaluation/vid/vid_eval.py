@@ -7,11 +7,16 @@ ignore lists are concatenated over the dataset, sorted by score, and turned into
 area-under-curve AP. What differs is where the time goes: the matching loops, which the reference runs in Python for every
 (image, class, detection, box), are one native call per (image, class) (`mega_vid_match_host` in libmega_b200.so), and
 the per-image bookkeeping is array code. Precision / recall / AP arrays equal the reference's element for element
-(tests/test_vid_eval_cpu.py runs both on the same synthetic detections)."""
+(tests/test_vid_eval_cpu.py runs both on the same synthetic detections).
+
+Proposal recall (box_only, the evaluation of an MODEL.RPN_ONLY run, vid_eval.py:72-119) runs on the GPU: the whole
+dataset is one launch of the kernel of csrc/proposal_recall.cu, one CTA per image, instead of the reference's Python loop
+of torch calls per greedy round and image."""
 import os
 from collections import defaultdict
 
 import numpy as np
+import torch
 
 from ..... import _lib
 
@@ -118,15 +123,85 @@ def eval_detection_vid(pred_boxlists, gt_boxlists, iou_thresh=0.5, motion_ranges
     return result
 
 
+def _pack(parts, out):
+    """concatenate per-image fp32 tensors into `out` (a view of the pinned staging buffer)"""
+    if parts:
+        torch.cat([p.detach().reshape(-1).float().cpu() for p in parts], out=out.view(-1))
+
+
+def _align(n, a=16):
+    return (n + a - 1) // a * a
+
+
+def _device():
+    if not torch.cuda.is_available():
+        raise _lib.MegaError("proposal recall runs on the GPU kernel of libmega_b200 only; no CUDA device is available")
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def proposal_recall(pred_boxlists, gt_boxlists, iou_thresh=0.5, limit=300):
+    """the device half of eval_proposals_vid -> (hits, num_pos, gt_overlaps [sum G] fp32 on the host): the inputs packed
+    into one pinned buffer, one host-to-device copy, one launch, one device-to-host copy of the counts and overlaps.
+    gt_overlaps holds, per image and in GT order, the greedy rounds' overlaps followed by zeros; it is 0 throughout for
+    images without GT or proposals, which the reference leaves out."""
+    from .....b200 import ops
+    assert len(gt_boxlists) == len(pred_boxlists), "Length of gt and pred lists need to be same."
+    dev = _device()
+    preds = [p.convert("xyxy") for p in pred_boxlists]
+    gts = [g.convert("xyxy") for g in gt_boxlists]
+    n = len(preds)
+    p_cnt = [len(p) for p in preds]
+    g_cnt = [len(g) for g in gts]
+    p_tot, g_tot = sum(p_cnt), sum(g_cnt)
+    sizes = [4 * 4 * p_tot, 4 * p_tot, 4 * 4 * g_tot, 8 * (n + 1), 8 * (n + 1)]
+    offs = [0]
+    for b in sizes:
+        offs.append(offs[-1] + _align(b))
+    host = torch.empty(offs[-1], dtype=torch.uint8, pin_memory=dev.type == "cuda")
+    view = lambda i, dtype, shape: host[offs[i]:offs[i] + sizes[i]].view(dtype).view(*shape)   # noqa: E731
+    _pack([p.bbox for p in preds], view(0, torch.float32, (p_tot, 4)))
+    _pack([p.get_field("objectness") for p in preds], view(1, torch.float32, (p_tot,)))
+    _pack([g.bbox for g in gts], view(2, torch.float32, (g_tot, 4)))
+    view(3, torch.int64, (n + 1,)).copy_(torch.tensor([0] + p_cnt, dtype=torch.int64).cumsum(0))
+    view(4, torch.int64, (n + 1,)).copy_(torch.tensor([0] + g_cnt, dtype=torch.int64).cumsum(0))
+    buf = host.to(dev, non_blocking=True)
+    dview = lambda i, dtype, shape: buf[offs[i]:offs[i] + sizes[i]].view(dtype).view(*shape)   # noqa: E731
+    out = torch.empty(24 + _align(4 * g_tot), dtype=torch.uint8, device=dev)
+    stats, overlaps = out[:24].view(torch.int64), out[24:24 + 4 * g_tot].view(torch.float32)
+    ops.proposal_recall(dview(0, torch.float32, (p_tot, 4)), dview(1, torch.float32, (p_tot,)),
+                        dview(3, torch.int64, (n + 1,)), dview(2, torch.float32, (g_tot, 4)),
+                        dview(4, torch.int64, (n + 1,)), max(p_cnt + [0]), max(g_cnt + [0]), limit, iou_thresh,
+                        overlaps, stats)
+    res = out.cpu()
+    hits, num_pos, rejected = res[:24].view(torch.int64).tolist()
+    assert rejected == 0, "proposal_recall: %d images exceed the packed bounds" % rejected
+    return hits, num_pos, res[24:24 + 4 * g_tot].view(torch.float32)
+
+
+def eval_proposals_vid(pred_boxlists, gt_boxlists, iou_thresh=0.5, limit=300):
+    """vid_eval.py:72-119: per image the proposals sorted by `objectness` (descending), the first `limit` of them
+    matched one to one with the GT boxes, greedily by largest IoU; recall = matched overlaps >= iou_thresh over all GT.
+    -> {"recall": float32 tensor}. GPU only: without a CUDA device this raises."""
+    hits, num_pos, _ = proposal_recall(pred_boxlists, gt_boxlists, iou_thresh, limit)
+    return {"recall": torch.tensor(float(hits), dtype=torch.float32) / float(num_pos)}
+
+
 def do_vid_evaluation(dataset, predictions, output_folder, box_only, motion_specific, logger):
-    """vid_eval.py:14-69 (detection branch; proposal recall -- box_only -- is outside the inference path)"""
-    if box_only:
-        raise NotImplementedError("proposal-recall evaluation is not part of the B200 build")
+    """vid_eval.py:14-69; box_only (the proposals of an MODEL.RPN_ONLY run): proposal recall, logged and written to
+    proposal_result.txt, returns None"""
     preds, gts = [], []
     for image_id, prediction in enumerate(predictions):
         info = dataset.get_img_info(image_id)
         preds.append(prediction.resize((info["width"], info["height"])))
         gts.append(dataset.get_groundtruth(image_id))
+    if box_only:
+        result = eval_proposals_vid(preds, gts, iou_thresh=0.5)
+        text = "Recall: {:.4f}".format(result["recall"])
+        logger.info(text)
+        if output_folder:
+            with open(os.path.join(output_folder, "proposal_result.txt"), "w") as fid:
+                fid.write(text)
+        return None
     ranges = [[0.0, 1.0], [0.0, 0.7], [0.7, 0.9], [0.9, 1.0]] if motion_specific else [[0.0, 1.0]]
     names = ["all", "fast", "medium", "slow"][:len(ranges)]
     result = eval_detection_vid(preds, gts, 0.5, ranges, motion_specific, False)

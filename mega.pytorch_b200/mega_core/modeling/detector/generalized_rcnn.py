@@ -7,7 +7,8 @@ GeneralizedRCNNFGFA   -- detector/generalized_rcnn_fgfa.py:19-219 (flow-guided a
 GeneralizedRCNNDFF    -- detector/generalized_rcnn_dff.py:19-138 (key-frame features warped along FlowNetS flow)
 
 `forward(images)` returns `list[BoxList]` (fields `scores`, `labels`) exactly like the reference in
-eval mode; the arithmetic runs in the B200 engine built lazily from this module's own state_dict
+eval mode -- under MODEL.RPN_ONLY (single-frame, FGFA and DFF) the proposals instead, field `objectness`, in descending
+objectness order (generalized_rcnn.py:51-55, rpn/rpn.py:186-197); the arithmetic runs in the B200 engine built lazily from this module's own state_dict
 (so weights loaded with load_state_dict / DetectronCheckpointer are what the kernels use).
 """
 import torch
@@ -29,7 +30,8 @@ class _EngineBacked(nn.Module):
         self.backbone = build_backbone(cfg)
         self.rpn = build_rpn(cfg, self.backbone.out_channels)
         self.roi_heads = build_roi_heads(cfg, self.backbone.out_channels)
-        for sub in (self.backbone, self.rpn, self.roi_heads["box"].feature_extractor):
+        extractor = (self.roi_heads["box"].feature_extractor,) if self.roi_heads else ()
+        for sub in (self.backbone, self.rpn) + extractor:
             if hasattr(sub, "_bind"):        # callable sub-modules (model.rpn(...), feature_extractor(..., pre_calculate=True))
                 sub._bind(self)
         self._engine = None
@@ -56,6 +58,10 @@ class _EngineBacked(nn.Module):
     def _to_boxlist(self, det, im_w, im_h):
         n = int(det.count.item())
         out = BoxList(det.boxes[:n].clone(), (int(im_w), int(im_h)), mode="xyxy")
+        if isinstance(det, _engine.Proposals):
+            out.add_field("objectness", det.objectness[:n].clone())
+            self.d2h_bytes_per_frame = 4 + n * (16 + 4)
+            return out
         out.add_field("scores", det.scores[:n].clone())
         out.add_field("labels", det.labels[:n].clone())
         self.d2h_bytes_per_frame = 4 + n * (16 + 4 + 8)

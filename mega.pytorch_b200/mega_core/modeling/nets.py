@@ -358,6 +358,10 @@ def build_rpn(cfg, in_channels):
 
 
 def build_roi_heads(cfg, in_channels):
+    """roi_heads.py:58-76: under MODEL.RPN_ONLY no head at all (an empty list, falsy like the reference's), so the model's
+    state_dict holds no roi_heads.* entries and the detector returns the RPN's proposals"""
+    if cfg.MODEL.RPN_ONLY:
+        return []
     return CombinedROIHeads(cfg, [("box", ROIBoxHead(cfg, in_channels))])
 
 
@@ -401,6 +405,17 @@ def engine_config_from(cfg):
         if att.ADVANCED_STAGE not in (0, 1):
             unsupported.append("MODEL.VID.ROI_BOX_HEAD.ATTENTION.ADVANCED_STAGE = %d (RdnEngine runs 0 or 1 advanced "
                                "stages)" % att.ADVANCED_STAGE)
+    if m.RPN_ONLY:
+        if v.METHOD in ("mega", "rdn"):
+            unsupported.append("MODEL.RPN_ONLY with MODEL.VID.METHOD '%s' (its test path reads the box head's feature "
+                               "extractor, which an RPN-only model does not have; served for 'base', 'dff' and 'fgfa')"
+                               % v.METHOD)
+        if cfg.TEST.BBOX_AUG.ENABLED:
+            unsupported.append("MODEL.RPN_ONLY with TEST.BBOX_AUG.ENABLED (test-time augmentation merges class "
+                               "detections, an RPN-only model returns proposals)")
+        if "B200" in m and m.B200.SEQ_NMS.ENABLED:
+            unsupported.append("MODEL.RPN_ONLY with MODEL.B200.SEQ_NMS.ENABLED (Seq-NMS links and rescores class "
+                               "detections by `scores` and `labels`, which proposals do not carry)")
     if unsupported:
         raise NotImplementedError("mega_core (B200 build): " + "; ".join(unsupported))
     # the reference sizes the long-range memory deques with ALL_FRAME_INTERVAL (roi_box_feature_extractors.py:660-668:
@@ -419,4 +434,5 @@ def engine_config_from(cfg):
         bbox_reg_weights=tuple(m.ROI_HEADS.BBOX_REG_WEIGHTS), anchor_sizes=tuple(m.RPN.ANCHOR_SIZES),
         aspect_ratios=tuple(m.RPN.ASPECT_RATIOS), anchor_stride=m.RPN.ANCHOR_STRIDE[0],
         num_classes=m.ROI_BOX_HEAD.NUM_CLASSES,
-        precision=os.environ.get("MEGA_B200_PRECISION", m.B200.PRECISION if "B200" in m else "f16"))
+        precision=os.environ.get("MEGA_B200_PRECISION", m.B200.PRECISION if "B200" in m else "f16"),
+        **({"rpn_only": True} if m.RPN_ONLY else {}))

@@ -6,7 +6,9 @@ The reference moves the per-rank `{image_id: BoxList}` dicts to rank 0 by pickli
 through the pickler twice and through a padded byte all-gather. `gather_predictions` sends the same information as five
 flat tensors (ids, sizes, counts, boxes | scores, labels) with two size exchanges and padded `all_gather`s of typed
 tensors -- no pickling, works with NCCL (device tensors) and gloo (CPU tensors) alike -- and returns the reference's
-result: on rank 0 the list of BoxLists ordered by image id, None elsewhere."""
+result: on rank 0 the list of BoxLists ordered by image id, None elsewhere. The proposals of an MODEL.RPN_ONLY run
+(BoxLists whose only field is `objectness`) travel the same way as four flat tensors (ids, sizes, counts, boxes |
+objectness)."""
 import logging
 import pickle
 
@@ -60,9 +62,48 @@ def all_gather(data):
     return [pickle.loads(p.numpy().tobytes()) for p in _gather_var(buf, dev)]
 
 
+def _objectness_only(predictions):
+    """True when the predictions are proposals (field `objectness`, no `scores`) on any rank"""
+    b = next(iter(predictions.values()), None)
+    flag = int(b is not None and b.has_field("objectness") and not b.has_field("scores"))
+    if get_world_size() > 1:
+        t = torch.tensor([flag], dtype=torch.int64, device=_comm_device())
+        dist.all_reduce(t, op=dist.ReduceOp.MAX)
+        flag = int(t.item())
+    return bool(flag)
+
+
+def _gather_proposals(predictions):
+    ids = sorted(predictions.keys())
+    boxlists = [predictions[i].convert("xyxy") for i in ids]
+    meta = torch.tensor([[i, b.size[0], b.size[1], len(b)] for i, b in zip(ids, boxlists)], dtype=torch.int64).reshape(-1, 4)
+    floats = torch.cat([torch.cat([b.bbox.float().cpu().reshape(-1, 4),
+                                   b.get_field("objectness").float().cpu().reshape(-1, 1)], 1)
+                        for b in boxlists]) if boxlists else torch.zeros(0, 5)
+    if get_world_size() > 1:
+        dev = _comm_device()
+        metas, floatss = _gather_var(meta, dev), _gather_var(floats, dev)
+    else:
+        metas, floatss = [meta], [floats]
+    if not is_main_process():
+        return None
+    merged = {}
+    for m, f in zip(metas, floatss):
+        off = 0
+        for image_id, w, h, n in m.tolist():
+            b = BoxList(f[off:off + n, :4].clone(), (w, h), mode="xyxy")
+            b.add_field("objectness", f[off:off + n, 4].clone())
+            merged[image_id] = b
+            off += n
+    return [merged[i] for i in sorted(merged.keys())]
+
+
 def gather_predictions(predictions):
     """{image_id: BoxList with `scores`, `labels`} per rank -> on rank 0 the list of BoxLists ordered by image id (what
-    engine/inference.py:50-69 returns), None on the other ranks"""
+    engine/inference.py:50-69 returns), None on the other ranks. BoxLists with the single field `objectness` (the
+    proposals of an RPN-only model) are gathered as such."""
+    if _objectness_only(predictions):
+        return _gather_proposals(predictions)
     ids = sorted(predictions.keys())
     boxlists = [predictions[i].convert("xyxy") for i in ids]
     meta = torch.tensor([[i, b.size[0], b.size[1], len(b)] for i, b in zip(ids, boxlists)], dtype=torch.int64).reshape(-1, 4)
