@@ -49,6 +49,9 @@ constexpr int kMaxCtas = 132;   // persistent grid: one CTA per SM of an H100 SX
 // four epilogue warps (one per 32-row quarter) and produced in column order, tile after tile.
 constexpr int kRingSlots = 2;
 constexpr int kRingSlotBytes = kBM * 128;
+// 3xFP16 holds a whole tile in its ring (chunk c of every tile in slot c), so that the MMA warpgroups hand over a finished
+// tile without waiting for the epilogue of the one before; the epilogue writes its result in place, into the rows it read.
+__host__ __device__ constexpr int ring_slots(int mode, int bn) { return mode == kModeF16x3 ? bn / 32 : kRingSlots; }
 __host__ __device__ constexpr int mma_warp0(int mode) { return mode == kModeSplit3 ? 12 : 8; }
 __host__ __device__ constexpr int conv_gemm_threads(int mode) { return (mma_warp0(mode) + 8) * 32; }
 // 3xFP16 registers per thread of warpgroup 0 (producer), 1 (epilogue) and 2-3 (MMA): the 64K registers of the SM
@@ -63,7 +66,7 @@ __host__ __device__ constexpr int pass_n(int bn) { return bn <= 128 ? bn : (bn =
 // fit the 227 KB of shared memory next to the ring and the epilogue staging.
 constexpr int conv_gemm_stages(int mode, int bn) {
   if (mode == kModeSplit3) return bn == 64 ? 4 : 2;
-  if (mode == kModeF16x3) return bn == 64 ? 5 : 4;
+  if (mode == kModeF16x3) return bn == 64 ? 6 : 4;
   return bn == 32 ? 6 : bn == 64 ? 5 : bn <= 128 ? 4 : bn <= 192 ? 3 : 2;
 }
 
@@ -114,9 +117,9 @@ struct SmemLayout {
   // 3xTF32: [A raw | B hi (masked in place by the splitters) | B lo]; the MMA warpgroups split A in registers
   static constexpr int kStageBytes = SPLIT3 ? kHalf + kBBytes : kHalf;
   static constexpr int kRingOffset = STAGES * kStageBytes;
-  static constexpr int kEpiOffset = kRingOffset + kRingSlots * kRingSlotBytes;   // 4 warps x (2 out + 2 residual) x 4 KB
-                                                                                 // (3xFP16: 4 warps x 4 chunks x 4 KB)
-  static constexpr int kEpiBytes = 4 * 4 * 4096;
+  static constexpr int kEpiOffset = kRingOffset + ring_slots(MODE, BN) * kRingSlotBytes;
+  // 4 warps x (2 out + 2 residual) x 4 KB (3xFP16: 4 warps x 2 residual x 4 KB; its results go back into the ring)
+  static constexpr int kEpiBytes = MODE == kModeF16x3 ? 4 * 2 * 4096 : 4 * 4 * 4096;
   static constexpr int kBarOffset = kEpiOffset + kEpiBytes;
   static constexpr int kSbCols = BN <= 128 ? 128 : 256;
   static constexpr int kSbOffset = kBarOffset + 512;              // [scale | bias][kSbCols] floats of the tile being finished
@@ -182,6 +185,15 @@ struct WorkIter {
     kb1 = KB;
     tile += grid;
     return true;
+  }
+  // the tile of the item next() returns next
+  __device__ __forceinline__ bool peek(int& t) const {
+    if (sk) {
+      t = u / KB;
+      return u < u_end;
+    }
+    t = tile;
+    return tile < tiles;
   }
 };
 
@@ -293,6 +305,14 @@ __device__ __forceinline__ void stage_scale_bias(float* sb, int bias_off, const 
   sb[i] = (p.scale && n < p.cout) ? __ldg(p.scale + zoff + n) : 1.f;
   sb[bias_off + i] = (p.bias && n < p.cout) ? __ldg(p.bias + zoff + n) : 0.f;
 }
+
+// 4 bytes from global to shared memory without a register in between (cp.async); zero-filled unless `valid`, in which case
+// nothing is read from src. Complete for the issuing thread after cp_async_wait_all.
+__device__ __forceinline__ void cp_async_f32(float* dst, const float* src, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(valid ? 4 : 0)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // ------------------------------------------------------------------ TMA producer
 struct PipeState {
@@ -534,8 +554,16 @@ __device__ __forceinline__ void mma_kblock_grouped(float (&d)[32], uint32_t a_ad
 struct MmaState {
   int stage;
   uint32_t phase;
-  uint32_t uses[kRingSlots];   // accumulator chunks handed to each ring slot so far
+  uint32_t uses[kRingSlots];   // accumulator chunks handed to each ring slot so far (3xFP16: uses[0] counts whole tiles)
 };
+
+// 3xFP16: the two MMA warpgroups issue their k-blocks in turn (named barriers 2 and 3 of the 256 MMA threads). Warpgroup 1
+// issues k-block n after warpgroup 0 has issued it, and warpgroup 0 issues k-block n + 1 after warpgroup 1 has issued n, so
+// the tensor pipe runs their MMAs one k-block apart: at every segment end one warpgroup folds into its master accumulator
+// while the other's MMAs keep the pipe busy. Warpgroup 1 arrives once before its first k-block and warpgroup 0 waits once
+// after its last, so that every arrival is matched.
+__device__ __forceinline__ void mma_turn_wait(int wg) { asm volatile("bar.sync %0, 256;" ::"r"(3 - wg)); }
+__device__ __forceinline__ void mma_turn_pass(int wg) { asm volatile("bar.arrive %0, 256;" ::"r"(2 + wg)); }
 
 // The MMAs of one work item (k-blocks [kb0, kb1)) for PN columns of the tile (one pass), by MMA warpgroup wg; the result
 // goes to the ring in 32-column chunks. SPLIT3 / 3xFP16 restart the accumulator every seg_len k-blocks and fold the segments
@@ -568,11 +596,13 @@ __device__ __forceinline__ void mma_pass(uint8_t* smem, uint64_t* full_bar, uint
     for (int kb = s0; kb < s1; ++kb) {
       mbar_wait(SPLIT3 ? &split_bar[ms.stage] : &full_bar[ms.stage], ms.phase);
       const uint32_t a_addr = smem_u32(smem + ms.stage * L::kStageBytes);
+      if constexpr (MODE == kModeF16x3) mma_turn_wait(wg);
       if constexpr (GW > 0)
         mma_kblock_grouped<MODE, GW>(d, a_addr + wg * 64 * 128, a_addr + L::kABytes, a_addr + L::kABytes + L::kBBytes, wtid,
                                      kb);
       else
         mma_kblock<PN, MODE>(d, a_addr + wg * 64 * 128, a_addr + L::kABytes, a_addr + L::kABytes + L::kBBytes, wtid, kb == s0);
+      if constexpr (MODE == kModeF16x3) mma_turn_pass(wg);
       // SPLIT3 reads its A fragments into registers for every k-block: nothing stays in flight across them
       if (SPLIT3) wgmma_wait<0>(); else wgmma_wait<1>();
       if (pending >= 0) {
@@ -603,14 +633,20 @@ __device__ __forceinline__ void mma_pass(uint8_t* smem, uint64_t* full_bar, uint
       has_master = true;
     }
   }
+  if constexpr (MODE == kModeF16x3) {   // chunk c of the tile -> slot c (the ring holds a whole tile)
 #pragma unroll
-  for (int c = 0; c < PN / 32; ++c) {
-    uint32_t slot;
-    if (hpc == 0) slot = (ms.uses[0] == ms.uses[1]) ? 0u : 1u;    // alternate
-    else slot = static_cast<uint32_t>((c / hpc) & 1);
-    const uint32_t use = ms.uses[slot]++;
-    if constexpr (SEG) ring_put(ring, ring_full, ring_empty, slot, use, wg, wtid, master, c);
-    else ring_put(ring, ring_full, ring_empty, slot, use, wg, wtid, d, c);
+    for (int c = 0; c < PN / 32; ++c) ring_put(ring, ring_full, ring_empty, c, ms.uses[0], wg, wtid, master, c);
+    ++ms.uses[0];
+  } else {
+#pragma unroll
+    for (int c = 0; c < PN / 32; ++c) {
+      uint32_t slot;
+      if (hpc == 0) slot = (ms.uses[0] == ms.uses[1]) ? 0u : 1u;    // alternate
+      else slot = static_cast<uint32_t>((c / hpc) & 1);
+      const uint32_t use = ms.uses[slot]++;
+      if constexpr (SEG) ring_put(ring, ring_full, ring_empty, slot, use, wg, wtid, master, c);
+      else ring_put(ring, ring_full, ring_empty, slot, use, wg, wtid, d, c);
+    }
   }
 }
 
@@ -640,6 +676,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr int kBK = mode_bk(MODE);
   constexpr int CW = OUTH ? 64 : 32;   // epilogue chunk: columns per 128-byte output row segment
   constexpr int kMmaWarp0 = mma_warp0(MODE);
+  constexpr int RS = ring_slots(MODE, BN);
   static_assert(!OUTH || BN % 64 == 0, "fp16 output needs block_n % 64 == 0");
   static_assert(SmemLayout<BN, STAGES, MODE>::kTotal <= 227 * 1024, "pipeline + staging exceed the 227 KB of a CTA");
   using L = SmemLayout<BN, STAGES, MODE>;
@@ -655,9 +692,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* split_bar = empty_bar + STAGES;       // [STAGES] (3xTF32 only)
-  uint64_t* ring_full = split_bar + STAGES;       // [kRingSlots]
-  uint64_t* ring_empty = ring_full + kRingSlots;  // [kRingSlots]
-  uint64_t* res_bar = ring_empty + kRingSlots;    // [4 warps][2] (3xFP16: [4 warps][4 chunks])
+  uint64_t* ring_full = split_bar + STAGES;       // [RS]
+  uint64_t* ring_empty = ring_full + RS;          // [RS]
+  uint64_t* res_bar = ring_empty + RS;            // [4 warps][2]
   int* epi_flag = reinterpret_cast<int*>(res_bar + 16);
   uint8_t* ring = smem + L::kRingOffset;
 
@@ -680,7 +717,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       mbar_init(&empty_bar[s], 8);      // one arrival per MMA warp
       mbar_init(&split_bar[s], 4);
     }
-    for (int b = 0; b < kRingSlots; ++b) {
+    for (int b = 0; b < RS; ++b) {
       mbar_init(&ring_full[b], 256);    // every MMA thread
       mbar_init(&ring_empty[b], 4);     // the four epilogue warps that read a slot
     }
@@ -717,6 +754,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     WorkIter it(p, PK ? ctaid_x_here() : cta, grid);
     int t;
     int kb0, kb1;
+    if (PK && wg == 1) mma_turn_pass(wg);
     while (it.next(t, kb0, kb1)) {
       mma_pass<P0, STAGES, MODE, L, GW>(smem, full_bar, empty_bar, split_bar, ring, ring_full, ring_empty, ms, kb0, kb1,
                                         kSegLen, wg, wtid, 0);
@@ -724,6 +762,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         mma_pass<P1, STAGES, MODE, L>(smem, full_bar, empty_bar, split_bar, ring, ring_full, ring_empty, ms, kb0, kb1,
                                       kSegLen, wg, wtid, 0);
     }
+    if (PK && wg == 0) mma_turn_wait(wg);
   } else if (warp >= 6 && warp < 10 && !PK) {
     // ===================== operand splitter (3xTF32 only, warps 6..9) =====================
     // B: hi = x truncated to TF32 written back in place, lo = x - hi into the region behind the raw tile (pre-split weights
@@ -766,27 +805,28 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   } else if (PK && warp >= 4 && warp < 8) {
     // ===================== epilogue, 3xFP16 (warps 4..7) =====================
     // One warp per 32-row quarter of the tile finishes all of its 32-column chunks: every ring slot is read by all four
-    // warps. The BN scale is folded into the packed weights, the bias slice of the NEXT tile is fetched during the current
-    // one (double-buffered, one barrier per tile), and the residual lands in the store staging buffer itself (every thread
-    // reads its 128-byte row into registers before it writes the same row), issued for all chunks at the start of the tile.
+    // warps. The BN scale is folded into the packed weights, and the bias slice of the NEXT tile is fetched during the
+    // current one (double-buffered, one barrier per tile). The ring holds the whole tile (chunk j in slot j): each warp
+    // writes its result back into the rows of the slot it read (every thread reads its 128-byte row into registers before
+    // it writes the same row), stores it from there, and hands the tile's slots back once those stores have read them. The
+    // residual arrives in two 4 KB buffers per warp: chunks 0 and 1 at the start of the tile, chunk j + 2 once j is read.
     setmaxnreg_dec<kF16x3RegsEpilogue>();
     constexpr int kCPW = BN / 32;          // 32-column chunks per warp
     const int q = warp & 3;                // 32-row quarter of the tile
     const int row = q * 32 + lane;
     const int epi_tid = (warp - 4) * 32 + lane;                              // 0 .. 127
-    uint8_t* stage_buf = smem + L::kEpiOffset + (warp - 4) * (kCPW * 4096);  // kCPW x 4 KB: residual in, result out
-    uint64_t* rbar = res_bar + (warp - 4) * 4;
+    uint8_t* res_buf = smem + L::kEpiOffset + (warp - 4) * 8192;             // 2 x 4 KB residual staging
+    uint64_t* rbar = res_bar + (warp - 4) * 2;
     float* bias_s = reinterpret_cast<float*>(smem + L::kSbOffset);           // [2][BN]
     uint32_t rphase = 0;
     const int cta_e = ctaid_x_here();
     WorkIter it(p, cta_e, grid);
     int t;
     int kb0, kb1;
-    uint32_t seq0 = 0;    // ring chunk number of this item's column 0
     const uint32_t sw = static_cast<uint32_t>(lane & 7);
     const bool res_split = p.res_split != 0;
     const float slope = p.relu == 2 ? 0.1f : 0.f;
-    for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item, seq0 += BN / 32) {
+    for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item) {
       const TileCoord tc = decode_tile(p, t, BN);
       const bool complete = (kb0 == 0 && kb1 == KB);
       const StoreBox box = store_box(p, tc, q);
@@ -801,39 +841,39 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
         epi_bar_sync<128>();
       }
-      float next_bias = 0.f;
-      bool has_next = false;
-      {
-        WorkIter peek = it;
-        int t2, k0, k1;
-        has_next = peek.next(t2, k0, k1);
-        if (has_next && epi_tid < BN) {
+      {   // the next tile's slice into [bsel ^ 1], which no warp reads before the next tile's barrier
+        int t2;
+        if (it.peek(t2) && epi_tid < BN) {
           const TileCoord tc2 = decode_tile(p, t2, BN);
           const int n = tc2.n0 + epi_tid;
-          next_bias = (p.bias && n < p.cout) ? __ldg(p.bias + tc2.batch * p.bias_z_off + n) : 0.f;
+          const bool valid = p.bias && n < p.cout;
+          cp_async_f32(bias_s + (bsel ^ 1) * BN + epi_tid,
+                       valid ? p.bias + tc2.batch * p.bias_z_off + n : static_cast<const float*>(p.out_ptr), valid);
         }
       }
-      // ---- the staging buffers are free once the previous tile's stores have read them; then the residual may land there
-      if (lane == 0) tma_store_wait_read<0>();
-      __syncwarp();
-      auto issue_residual = [&]() {
-        if (p.has_residual && lane == 0) {
-#pragma unroll
-          for (int j = 0; j < kCPW; ++j) {
-            if (j < nchunks) {
-              mbar_arrive_expect_tx(&rbar[j], 4096);
-              tma_load_4d(stage_buf + j * 4096, &tmRes, &rbar[j], tc.n0 + j * 32 + tc.batch * p.res_c_off, box.w, box.h,
-                          box.res_n);
-            }
-          }
+      // ---- residual chunk j into buffer j & 1 (read by the time chunk j + 2 is issued: the reads precede a fence and a
+      //      __syncwarp)
+      const int res_c0 = tc.n0 + tc.batch * p.res_c_off;
+      auto issue_residual = [&](const int j) {
+        if (p.has_residual && lane == 0 && j < nchunks) {
+          mbar_arrive_expect_tx(&rbar[j & 1], 4096);
+          tma_load_4d(res_buf + (j & 1) * 4096, &tmRes, &rbar[j & 1], res_c0 + j * 32, box.w, box.h, box.res_n);
         }
       };
-      if (complete) issue_residual();
-      auto load_chunk = [&](const int j, float (&acc)[32]) {
-        uint32_t raw[32];
-        ring_take(ring, ring_full, ring_empty, seq0 + j, row, raw);
+      if (complete) {
+        issue_residual(0);
+        issue_residual(1);
+      }
+      // Every warp waits for every chunk of every tile, columns past cout included: a parity wait only tells the phase it
+      // names from its neighbours, so neither side may run more than one phase ahead of the other.
+      auto take_chunk = [&](const int j, uint32_t (&r)[32]) {
+        mbar_wait(&ring_full[j], bsel);
+        const uint8_t* rowp = ring + j * kRingSlotBytes + row * 128;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[i] = __uint_as_float(raw[i]);
+        for (int i = 0; i < 8; ++i) {
+          const uint4 v = *reinterpret_cast<const uint4*>(rowp + ((static_cast<uint32_t>(i) ^ sw) << 4));
+          r[4 * i] = v.x; r[4 * i + 1] = v.y; r[4 * i + 2] = v.z; r[4 * i + 3] = v.w;
+        }
       };
       bool finalize = complete;
       int c_first = cta_e, c_last = cta_e;
@@ -843,11 +883,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
         for (int j = 0; j < kCPW; ++j) {
           uint32_t raw[32];
-          ring_take(ring, ring_full, ring_empty, seq0 + j, row, raw);
+          take_chunk(j, raw);
           sk_publish(part, j * 32, raw);
         }
         finalize = sk_elect_finisher<128>(p, U, grid, KB, t, epi_tid, epi_flag, c_first, c_last);
-        if (finalize) issue_residual();
+        if (finalize) {
+          issue_residual(0);
+          issue_residual(1);
+        }
       }
       if (finalize) {
         const int out_n = tc.img + tc.batch * p.out_n_off;
@@ -855,9 +898,16 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int j = 0; j < kCPW; ++j) {
           if (j < nchunks) {
             float acc[32];
-            if (complete) load_chunk(j, acc);
-            else sk_reduce(p, U, grid, KB, t, c_first, c_last, row, BN, j * 32, acc);
-            uint8_t* rowp = stage_buf + j * 4096 + lane * 128;
+            if (complete) {
+              uint32_t raw[32];
+              take_chunk(j, raw);
+#pragma unroll
+              for (int i = 0; i < 32; ++i) acc[i] = __uint_as_float(raw[i]);
+            } else {
+              sk_reduce(p, U, grid, KB, t, c_first, c_last, row, BN, j * 32, acc);
+            }
+            uint8_t* rowp = ring + j * kRingSlotBytes + row * 128;        // the result goes back to the row it came from
+            const uint8_t* resp = res_buf + (j & 1) * 4096 + lane * 128;
             const float4* biv = reinterpret_cast<const float4*>(bias_s + bsel * BN + j * 32);
 #pragma unroll
             for (int i = 0; i < 32; i += 4) {
@@ -866,13 +916,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               acc[i + 2] = fmaf(acc[i + 2], p.acc_scale, bi.z); acc[i + 3] = fmaf(acc[i + 3], p.acc_scale, bi.w);
             }
             if (p.has_residual) {
-              mbar_wait(&rbar[j], (rphase >> j) & 1u);
-              rphase ^= (1u << j);
+              mbar_wait(&rbar[j & 1], (rphase >> (j & 1)) & 1u);
+              rphase ^= (1u << (j & 1));
               if (res_split) {    // 16-byte chunks 0..3: hi halves of values 8c .. 8c+7, chunks 4..7: their lo halves
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {
-                  const uint4 rh = *reinterpret_cast<const uint4*>(rowp + ((static_cast<uint32_t>(c) ^ sw) << 4));
-                  const uint4 rl = *reinterpret_cast<const uint4*>(rowp + ((static_cast<uint32_t>(4 + c) ^ sw) << 4));
+                  const uint4 rh = *reinterpret_cast<const uint4*>(resp + ((static_cast<uint32_t>(c) ^ sw) << 4));
+                  const uint4 rl = *reinterpret_cast<const uint4*>(resp + ((static_cast<uint32_t>(4 + c) ^ sw) << 4));
                   const uint32_t hs[4] = {rh.x, rh.y, rh.z, rh.w}, ls[4] = {rl.x, rl.y, rl.z, rl.w};
 #pragma unroll
                   for (int e = 0; e < 4; ++e) {
@@ -884,12 +934,11 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               } else {
 #pragma unroll
                 for (int c = 0; c < 8; ++c) {
-                  const float4 rr = *reinterpret_cast<const float4*>(rowp + ((static_cast<uint32_t>(c) ^ sw) << 4));
+                  const float4 rr = *reinterpret_cast<const float4*>(resp + ((static_cast<uint32_t>(c) ^ sw) << 4));
                   acc[4 * c] += rr.x; acc[4 * c + 1] += rr.y; acc[4 * c + 2] += rr.z; acc[4 * c + 3] += rr.w;
                 }
               }
             }
-            // (every read of the row precedes the first write below: the result goes back to the same bytes)
             if (p.relu) {
 #pragma unroll
               for (int i = 0; i < 32; ++i) acc[i] = fmaxf(acc[i], slope * acc[i]);
@@ -915,18 +964,26 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
             fence_async_smem();
             __syncwarp();
+            if (j + 2 < kCPW) issue_residual(j + 2);
             const int gc0 = tc.n0 + j * 32 + tc.batch * p.out_c_off;
             if (!OUT16 && gc0 + 32 > p.out_tail0) store_tail<false>(p, rowp, gc0, 32, box, out_n, lane);
             if (lane == 0 && gc0 < p.out_tail0) {
-              tma_store_4d(&tmOut, stage_buf + j * 4096, gc0, box.w, box.h, out_n);
+              tma_store_4d(&tmOut, ring + j * kRingSlotBytes + q * 4096, gc0, box.w, box.h, out_n);
               tma_store_commit();
             }
           } else if (complete) {
-            ring_skip(ring, ring_full, ring_empty, seq0 + j, row);   // columns past cout: hand the slot back unread
+            mbar_wait(&ring_full[j], bsel);   // columns past cout: nothing to read
           }
         }
       }
-      if (has_next && epi_tid < BN) bias_s[(bsel ^ 1) * BN + epi_tid] = next_bias;
+      // ---- the tile's slots go back to the MMA warpgroups once this warp's stores have read its rows
+      if (lane == 0) tma_store_wait_read<0>();
+      __syncwarp();
+      if (lane == 0) {
+#pragma unroll
+        for (int j = 0; j < kCPW; ++j) mbar_arrive(&ring_empty[j]);
+      }
+      cp_async_wait_all();
     }
     if (lane == 0) tma_store_wait<0>();   // global writes complete before the CTA retires
   } else if (PK) {

@@ -10,6 +10,12 @@ and its share of the device-timed step (CUDA graphs, device-resident inputs: the
 name / power limit / max SM clock. The JSON written with --json also holds a SHA-256 digest of the output tensor of every
 3xFP16 launch of one further step: two builds that compute the same bits give the same list.
 
+Each launch also gets its floor: the compute floor (executed fp16 products over the dense fp16 peak) and the HBM floor
+(bytes it must move over the HBM bandwidth; A once, B, the output and the residual, 4 bytes per value as in the
+split-fp16 format), which of the two bounds it, and the measured time over that floor. The peaks are bench.py's:
+MEASURED_PEAKS.json when present, else the H100 SXM data sheet. The 3xFP16 launches are then summed per layer family
+(stem, res2-4 1x1 and 3x3, RPN, res5, l_fcs[0], relation, predictor), named from the engine functions that made them.
+
 Tiles come from the fixed heuristic (MEGA_B200_AUTOTUNE=0), so every run launches the same kernels on the same shapes.
 The per-launch times come from eager launches (one event pair each, no overlap between kernels), the step time from graph
 replays in which consecutive kernels overlap (programmatic dependent launch), so the share can exceed 1.
@@ -44,16 +50,43 @@ def card():
     return out[idx].strip() if idx < len(out) else None
 
 
+FAMILY_OF = {"res5_reduced": "res5", "_reduce": "res5", "rpn_head": "RPN", "_fc0": "l_fcs[0]", "predict_gemm": "predictor",
+             "_attention": "relation", "aggregate": "relation", "_aggregate_split": "relation"}
+
+
+def family(frame, taps):
+    """layer family of a launch, from the engine functions on its call stack (innermost first); None if unknown"""
+    body = None
+    while frame is not None:
+        name, loc = frame.f_code.co_name, frame.f_locals
+        if name in FAMILY_OF:
+            return FAMILY_OF[name]
+        if name == "forward" and "si" in loc and "blk" in loc:     # ResNetStages.forward: res2-4, or res5 further out
+            body = "res2-4 %s" % ("1x1" if taps == 1 else "3x3")
+        elif name == "forward" and type(loc.get("self")).__name__ == "Backbone":
+            return body or "stem"
+        frame = frame.f_back
+    return body
+
+
+def launch_bytes(info):
+    """bytes a conv_gemm launch must move through HBM: A once, B, the output and the residual, 4 bytes per value"""
+    m = info["m"] * info["batch"]
+    n = m * info["k"] + info["batch"] * info["cout"] * info["k"] * info["taps"] + m * info["cout"] * (2 if info["res"] else 1)
+    return 4 * n
+
+
 def launch_times(step, reps):
-    """[(info, flops, ms averaged over reps)] for every tensor-core launch of one eager step"""
+    """[(info, flops, ms averaged over reps, layer family)] for every tensor-core launch of one eager step"""
     rec = []
 
     def hook(run, flops, info):
+        fam = family(sys._getframe(1), info.get("taps", 1))
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         run()
         b.record()
-        rec.append((a, b, flops, info))
+        rec.append((a, b, flops, info, fam))
 
     ops.TIMING_HOOK[0] = hook
     try:
@@ -67,7 +100,7 @@ def launch_times(step, reps):
         ops.TIMING_HOOK[0] = None
     n = len(rec) // reps
     assert n * reps == len(rec), "launch sequence differs between steps"
-    return [(rec[i][3], rec[i][2], sum(r[0].elapsed_time(r[1]) for r in rec[i::n]) / reps) for i in range(n)]
+    return [(rec[i][3], rec[i][2], sum(r[0].elapsed_time(r[1]) for r in rec[i::n]) / reps, rec[i][4]) for i in range(n)]
 
 
 def output_digests(step):
@@ -139,21 +172,28 @@ def main():
         finally:
             eng._graphs, eng.use_graph = graphs, True
 
+    pk = bench.peaks()
+    flop_rate, byte_rate = pk["tflops"] * 1e12, pk["hbm_gbs"] * 1e9
     rows = []
-    print("%4s %7s %5s %5s %4s %4s %3s %7s %9s %9s" % ("#", "m", "cout", "k", "taps", "bn", "sk", "prec", "ms", "TFLOP/s"))
-    for i, (info, flops, ms) in enumerate(launches):
+    print("%4s %7s %5s %5s %4s %4s %3s %7s %9s %9s %8s %9s %9s %5s %6s  %s" % (
+        "#", "m", "cout", "k", "taps", "bn", "sk", "prec", "ms", "TFLOP/s", "MB", "tc_ms", "hbm_ms", "bound", "x", "family"))
+    for i, (info, flops, ms, fam) in enumerate(launches):
         if "chain_layers" in info:
             row = {"kind": "conv_chain", "layers": info["chain_layers"], "ms": ms, "flops": flops, "executed_tflops": None}
             print("%4d conv_chain_kernel (%d layers) %34.4f" % (i, info["chain_layers"], ms))
         else:
             prec = PRECISION_NAME.get(info.get("precision"), "?")
             products = 3 if prec in ("3xFP16", "3xTF32") else 1
+            nbytes = launch_bytes(info)
+            tc_ms, hbm_ms = products * flops / flop_rate * 1e3, nbytes / byte_rate * 1e3
             row = {"kind": "conv_gemm", "m": info["m"] * info["batch"], "cout": info["cout"], "k": info["k"],
                    "taps": info["taps"], "block_n": info["bn"], "stream_k": info["sk"], "precision": prec, "ms": ms,
-                   "flops": flops, "executed_tflops": products * flops / (ms * 1e-3) / 1e12}
-            print("%4d %7d %5d %5d %4d %4d %3d %7s %9.4f %9.1f" % (i, row["m"], row["cout"], row["k"], row["taps"],
-                                                                 row["block_n"], row["stream_k"], prec, ms,
-                                                                 row["executed_tflops"]))
+                   "flops": flops, "executed_tflops": products * flops / (ms * 1e-3) / 1e12, "family": fam,
+                   "bytes": nbytes, "compute_floor_ms": tc_ms, "hbm_floor_ms": hbm_ms,
+                   "bound": "tc" if tc_ms >= hbm_ms else "hbm", "over_floor": ms / max(tc_ms, hbm_ms)}
+            print("%4d %7d %5d %5d %4d %4d %3d %7s %9.4f %9.1f %8.1f %9.4f %9.4f %5s %6.2f  %s" % (
+                i, row["m"], row["cout"], row["k"], row["taps"], row["block_n"], row["stream_k"], prec, ms,
+                row["executed_tflops"], nbytes / 1e6, tc_ms, hbm_ms, row["bound"], row["over_floor"], fam))
         rows.append(row)
     f16x3 = [r for r in rows if r.get("precision") == "3xFP16"]
     f16x3_ms = sum(r["ms"] for r in f16x3)
@@ -163,6 +203,25 @@ def main():
               "tensor_core_ms_per_step": kernel_ms, "f16x3_launches": len(f16x3), "f16x3_ms_per_step": f16x3_ms,
               "f16x3_share_of_step": f16x3_ms / step_ms, "f16x3_executed_tflops": exec_tflops,
               "launches": rows, "f16x3_output_sha256": digests}
+    fams = {}
+    for r in f16x3:
+        f = fams.setdefault(r["family"] or "other", {"launches": 0, "ms": 0.0, "floor_ms": 0.0, "compute_floor_ms": 0.0,
+                                                     "hbm_floor_ms": 0.0, "hbm_bound_launches": 0})
+        f["launches"] += 1
+        f["ms"] += r["ms"]
+        f["floor_ms"] += max(r["compute_floor_ms"], r["hbm_floor_ms"])
+        f["compute_floor_ms"] += r["compute_floor_ms"]
+        f["hbm_floor_ms"] += r["hbm_floor_ms"]
+        f["hbm_bound_launches"] += r["bound"] == "hbm"
+    result["f16x3_families"] = fams
+    result["peaks"] = pk
+    print("3xFP16 launches per layer family (floors from %s: %.0f TFLOP/s, %.0f GB/s)" % (pk["src"], pk["tflops"],
+                                                                                          pk["hbm_gbs"]))
+    print("%-12s %4s %9s %9s %9s %9s %6s %4s" % ("family", "n", "ms", "floor_ms", "tc_ms", "hbm_ms", "x", "hbm"))
+    for name, f in sorted(fams.items(), key=lambda kv: -kv[1]["ms"]):
+        print("%-12s %4d %9.3f %9.3f %9.3f %9.3f %6.2f %4d" % (name, f["launches"], f["ms"], f["floor_ms"],
+                                                              f["compute_floor_ms"], f["hbm_floor_ms"],
+                                                              f["ms"] / f["floor_ms"], f["hbm_bound_launches"]))
     print("card (name, power limit, max SM clock): %s" % result["card"])
     print("device-timed step: %.3f ms (%d key frames)  tensor-core launches: %d, %.3f ms" % (step_ms, fps, len(rows), kernel_ms))
     print("3xFP16 launches: %d, %.3f ms per step = %.1f %% of the step, %.1f executed TFLOP/s" % (
