@@ -517,6 +517,73 @@ int mega_proposal_recall(const float* prop_boxes, const float* prop_scores, cons
                          int limit, float iou_thresh, void* workspace, long long workspace_bytes, float* gt_overlaps,
                          unsigned long long* stats, void* stream);
 
+/* ------------------------------------------------------------- baseline JPEG decode (SURVEY.md section 8f row 1)
+ * Replaces `PIL.Image.open(path).convert("RGB")` of the reference's datasets (data/datasets/vid.py:95 and the frames
+ * the detectors open themselves) with the SAME uint8 pixels, produced on the device: libjpeg's defaults as Pillow
+ * uses them -- integer "slow" IDCT, triangle-filter ("fancy") chroma upsampling, 16-bit fixed-point YCbCr -> RGB.
+ * The format splits the work: marker parsing and Huffman decoding are serial and run on the host
+ * (mega_jpeg_probe / mega_jpeg_entropy_decode: HOST functions, every pointer a host pointer, no CUDA call, safe to
+ * call from several threads); dequantisation, IDCT, upsampling and colour conversion run in two kernels that serve a
+ * whole batch of images of different sizes (mega_jpeg_decode_batch).
+ *
+ * Supported: SOF0 / 8-bit Huffman SOF1, 1 or 3 components, luma sampling 1x1 / 2x1 / 2x2 with 1x1 chroma, one
+ * interleaved scan or one scan per component, DRI / RSTn, 8- and 16-bit DQT. Anything else -- progressive, arithmetic,
+ * 12-bit, 4 components, other sampling factors -- returns MEGA_JPEG_UNSUPPORTED; a truncated or damaged stream (data
+ * that runs out, an invalid Huffman code or a table libjpeg refuses, restart markers out of sequence, no EOI after
+ * the last scan, a block whose coefficients leave the range in which libjpeg's 16-bit SIMD IDCT is reproduced)
+ * returns MEGA_JPEG_CORRUPT: the caller lets Pillow decide those. Neither reads or writes outside the buffers it was given. */
+#define MEGA_JPEG_UNSUPPORTED 16
+#define MEGA_JPEG_CORRUPT 17
+#define MEGA_JPEG_GREY 0
+#define MEGA_JPEG_YCBCR 1
+#define MEGA_JPEG_RGB 2
+
+/* one image as the host stage describes it. Component c has hmax x vmax (c == 0) or 1 x 1 samples per MCU; comp_dw /
+ * comp_dh its true size ceil(width * h / hmax) x ceil(height * v / vmax); comp_bw / comp_bh its 8x8-block grid padded
+ * to whole MCUs; its blocks are rows of that grid starting at block comp_block_off[c] of the image's coefficients. */
+typedef struct mega_jpeg_info {
+  int width, height, ncomp;
+  int hmax, vmax;                /* luma sampling factors: 1x1 (4:4:4, greyscale), 2x1 (4:2:2), 2x2 (4:2:0) */
+  int color;                     /* MEGA_JPEG_GREY / YCBCR / RGB, decided as libjpeg does (JFIF, Adobe, ids) */
+  int mcus_x, mcus_y;
+  int comp_dw[3], comp_dh[3], comp_bw[3], comp_bh[3];
+  long long comp_block_off[3];
+  long long total_blocks;        /* int16 coefficients needed: total_blocks * 64 */
+  unsigned short quant[3][64];   /* natural (row-major) order, as latched when the component's scan began */
+} mega_jpeg_info;
+
+/* one image of a batch as the kernels see it (mega_jpeg_plan_batch fills it; the caller uploads the array) */
+typedef struct mega_jpeg_desc {
+  int width, height, ncomp, hmax, vmax, color;
+  int comp_dw[3], comp_dh[3], comp_bw[3];
+  int quads_per_row;             /* ceil(width / 4): the colour kernel handles 4 pixels of a row per thread */
+  long long block_start;         /* first block of the image in the batch's coefficient / sample buffers */
+  long long comp_block_off[3];
+  long long total_blocks;
+  long long quad_start;          /* first colour work item of the image in the batch */
+  long long out_off;             /* byte offset of the image's [3, height, width] planes in `out` (16-byte aligned) */
+  unsigned short quant[3][64];
+} mega_jpeg_desc;
+
+/* parse the headers up to the first scan: geometry only (quant is not filled). */
+int mega_jpeg_probe(const unsigned char* data, long long size, mega_jpeg_info* info);
+/* full host stage: fills *info and writes the quantised coefficients, de-zigzagged (natural order), DC prediction
+ * undone, int16 [info->total_blocks, 64], into coef; coef_capacity_blocks (from the probe) bounds every write. */
+int mega_jpeg_entropy_decode(const unsigned char* data, long long size, mega_jpeg_info* info, short* coef,
+                             long long coef_capacity_blocks);
+/* HOST: lays n decoded images out as one batch. descs [n]; totals[0] = blocks (coefficient buffer: totals[0] * 64
+ * int16, image i at block descs[i].block_start; sample workspace: totals[0] * 64 bytes), totals[1] = colour work
+ * items, totals[2] = bytes of `out`. */
+int mega_jpeg_plan_batch(const mega_jpeg_info* infos, int n, mega_jpeg_desc* descs, long long* totals);
+/* DEVICE stage, two launches for the whole batch on the caller's stream; no allocation, no synchronisation.
+ * descs_host / descs_dev: the same n descriptors in host and in device memory; coef_dev: int16 [totals[0], 64];
+ * planes_dev: workspace of totals[0] * 64 bytes, 8-byte aligned (the component planes, padded to whole MCUs);
+ * out_dev: totals[2] bytes, 4-byte aligned; image i is planar uint8 [3, height, width] at descs[i].out_off -- the
+ * layout mega_image_transform_u8 consumes with src_pix_stride 1. */
+int mega_jpeg_decode_batch(const mega_jpeg_desc* descs_host, const mega_jpeg_desc* descs_dev, int n,
+                           const short* coef_dev, unsigned char* planes_dev, long long planes_bytes,
+                           unsigned char* out_dev, long long out_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

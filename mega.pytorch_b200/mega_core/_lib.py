@@ -243,6 +243,33 @@ lib.mega_proposal_recall_workspace_bytes.restype = _ll
 lib.mega_proposal_recall.argtypes = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _ll, _vp, _vp, _vp]
 lib.mega_proposal_recall.restype = _i
 
+
+class JpegInfo(ctypes.Structure):
+    """mirror of `mega_jpeg_info`"""
+    _fields_ = [("width", _i), ("height", _i), ("ncomp", _i), ("hmax", _i), ("vmax", _i), ("color", _i),
+                ("mcus_x", _i), ("mcus_y", _i), ("comp_dw", _i * 3), ("comp_dh", _i * 3), ("comp_bw", _i * 3),
+                ("comp_bh", _i * 3), ("comp_block_off", _ll * 3), ("total_blocks", _ll),
+                ("quant", (ctypes.c_ushort * 64) * 3)]
+
+
+class JpegDesc(ctypes.Structure):
+    """mirror of `mega_jpeg_desc`"""
+    _fields_ = [("width", _i), ("height", _i), ("ncomp", _i), ("hmax", _i), ("vmax", _i), ("color", _i),
+                ("comp_dw", _i * 3), ("comp_dh", _i * 3), ("comp_bw", _i * 3), ("quads_per_row", _i),
+                ("block_start", _ll), ("comp_block_off", _ll * 3), ("total_blocks", _ll), ("quad_start", _ll),
+                ("out_off", _ll), ("quant", (ctypes.c_ushort * 64) * 3)]
+
+
+JPEG_UNSUPPORTED, JPEG_CORRUPT = 16, 17
+lib.mega_jpeg_probe.argtypes = [ctypes.c_char_p, _ll, ctypes.POINTER(JpegInfo)]
+lib.mega_jpeg_probe.restype = _i
+lib.mega_jpeg_entropy_decode.argtypes = [ctypes.c_char_p, _ll, ctypes.POINTER(JpegInfo), _vp, _ll]
+lib.mega_jpeg_entropy_decode.restype = _i
+lib.mega_jpeg_plan_batch.argtypes = [ctypes.POINTER(JpegInfo), _i, ctypes.POINTER(JpegDesc), ctypes.POINTER(_ll)]
+lib.mega_jpeg_plan_batch.restype = _i
+lib.mega_jpeg_decode_batch.argtypes = [_vp, _vp, _i, _vp, _vp, _ll, _vp, _ll, _vp]
+lib.mega_jpeg_decode_batch.restype = _i
+
 EXPORTS = [
     "mega_last_error", "mega_abi_version", "mega_device_ok", "mega_conv_gemm", "mega_conv_gemm_tf32", "mega_conv_gemm_workspace_bytes", "mega_set_tf32_rounding",
     "mega_conv_chain_plan_bytes", "mega_conv_chain_encode", "mega_conv_chain_launch", "mega_conv_chain_set_trace",
@@ -260,4 +287,5 @@ EXPORTS = [
     "mega_seq_nms_workspace_bytes", "mega_seq_nms",
     "mega_image_transform_u8_ex", "mega_bbox_aug_workspace_bytes", "mega_bbox_aug_collect", "mega_bbox_aug_merge",
     "mega_proposal_recall_workspace_bytes", "mega_proposal_recall",
+    "mega_jpeg_probe", "mega_jpeg_entropy_decode", "mega_jpeg_plan_batch", "mega_jpeg_decode_batch",
 ]

@@ -130,7 +130,12 @@ _C = CfgNode({
         # SEQ_NMS (B200 build only): Seq-NMS over whole videos after the detection loop (mega_core.engine.seq_nms) --
         # boxes of consecutive frames link at IoU > LINK_IOU, a chain suppresses IoU > NMS_IOU in its frames, its boxes
         # get the chain's "avg" or "max" score
-        "B200": {"PRECISION": "f16",
+        # JPEG_DECODE (B200 build only): "pil" -- the datasets and the detectors' look-ahead reads decode frames with
+        # PIL on the host, as the reference does; "device" -- they read the file's bytes and the device transform
+        # decodes all frames of an item as one batch (mega_core.data.transforms.decode_jpeg_exact: Huffman decoding on
+        # host threads, IDCT / upsampling / colour conversion in CUDA, PIL's pixels bit for bit). TEST.BBOX_AUG keeps
+        # PIL either way: its collator hands PIL images to im_detect_bbox_aug, which transforms each pass itself
+        "B200": {"PRECISION": "f16", "JPEG_DECODE": "pil",
                  "SEQ_NMS": {"ENABLED": False, "LINK_IOU": 0.5, "NMS_IOU": 0.3, "RESCORE": "avg"}},
     },
     "INPUT": {"MIN_SIZE_TRAIN": (800,), "MAX_SIZE_TRAIN": 1333, "MIN_SIZE_TEST": 800, "MAX_SIZE_TEST": 1333,

@@ -15,6 +15,7 @@ from PIL import Image
 from ...config import cfg
 from ...structures.bounding_box import BoxList
 from ...utils.comm import is_main_process
+from ..transforms.jpeg import EncodedImage
 
 _NAMES = ("__background__ airplane antelope bear bicycle bird bus car cattle dog domestic_cat elephant fox giant_panda "
           "hamster horse lion lizard monkey motorcycle rabbit red_panda sheep snake squirrel tiger train turtle watercraft "
@@ -60,11 +61,18 @@ class VIDDataset(torch.utils.data.Dataset):
 
     # ---- images
     def _open(self, name):
+        if getattr(self.transforms, "jpeg_decode", "pil") == "device":       # MODEL.B200.JPEG_DECODE
+            with open(self._img_dir % name, "rb") as f:
+                return EncodedImage(f.read())
         return Image.open(self._img_dir % name).convert("RGB")
 
     def _transformed(self, idx, img, extra):
         """(current image, target) and every list of extra frames through the transform, as the reference's items do"""
         target = self.get_groundtruth(idx).clip_to_image(remove_empty=True)
+        if isinstance(img, EncodedImage):                   # every frame of the item in one decode batch
+            frames = self.transforms.decode_batch([img] + [f for k in extra for f in extra[k]])
+            img, rest = frames[0], iter(frames[1:])
+            extra = {k: [next(rest) for _ in extra[k]] for k in extra}
         if self.transforms is not None:
             img, target = self.transforms(img, target)
             extra = {k: [self.transforms(f, None)[0] for f in frames] for k, frames in extra.items()}

@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from ... import _lib
+from .jpeg import EncodedImage, decode_jpeg_exact
 
 PRECISION_BITS = 32 - 8 - 2
 
@@ -80,9 +81,15 @@ class DeviceTestTransform(object):
     """callable with the reference's transform signature `(image, target=None) -> (tensor, target)`.
     image: PIL.Image (RGB), uint8 ndarray / tensor [H, W, 3] on the host or on the device, or a planar uint8 [3, H, W]
     tensor (what `decode_jpeg` below / torchvision.io.decode_jpeg(device="cuda") returns: nvJPEG output is consumed in
-    place, no re-layout). Returns a float32 [3, H', W'] device tensor."""
+    place, no re-layout), or an `EncodedImage` (JPEG bytes, decoded on the device by `decode_jpeg_exact` to PIL's
+    pixels). Returns a float32 [3, H', W'] device tensor.
+    `jpeg_decode` ("pil" / "device", MODEL.B200.JPEG_DECODE) tells whoever opens the files -- the datasets and the
+    detectors' look-ahead reads -- what to hand over: a decoded PIL image, or the file's bytes through `decode_batch`."""
 
-    def __init__(self, min_size, max_size, mean, std, to_bgr255=True, device="cuda", hflip=False):
+    def __init__(self, min_size, max_size, mean, std, to_bgr255=True, device="cuda", hflip=False, jpeg_decode="pil"):
+        if jpeg_decode not in ("pil", "device"):
+            raise ValueError("MODEL.B200.JPEG_DECODE must be \"pil\" or \"device\", got %r" % (jpeg_decode,))
+        self.jpeg_decode = jpeg_decode
         if isinstance(min_size, (list, tuple)):
             assert len(min_size) == 1, "test-time transform: a single MIN_SIZE_TEST"
             min_size = min_size[0]
@@ -106,7 +113,16 @@ class DeviceTestTransform(object):
             self._tables[key] = t
         return t
 
+    def decode_batch(self, images):
+        """list of EncodedImage -> list of planar uint8 [3, H, W] tensors on the device, decoded as one batch (one
+        copy, two launches); an object that appears several times in the list is decoded once"""
+        uniq = list({id(e): e for e in images}.values())
+        decoded = dict(zip((id(e) for e in uniq), decode_jpeg_exact([e.data for e in uniq], device=self.device)))
+        return [decoded[id(e)] for e in images]
+
     def __call__(self, image, target=None, out=None):
+        if isinstance(image, EncodedImage):
+            image = decode_jpeg_exact(image.data, device=self.device)
         if not torch.is_tensor(image) and hasattr(image, "convert"):         # PIL.Image
             image = np.asarray(image.convert("RGB"))
         if isinstance(image, np.ndarray):

@@ -175,12 +175,23 @@ class GeneralizedRCNNMEGA(_EngineBacked):
     def _read_lookahead(self, infos, n):
         """frame 0 of a video: the reference opens the next frames from disk inside the model"""
         from PIL import Image
-        frames = []
+        names = []
         for _ in range(n):
             self.end_id = min(self.end_id + 1, self.seg_len - 1)
-            name = infos["pattern"] % self.end_id
-            img = Image.open(infos["img_dir"] % name).convert("RGB")
-            img = infos["transforms"](img)
+            names.append(infos["img_dir"] % (infos["pattern"] % self.end_id))
+        transform = infos["transforms"]
+        if getattr(transform, "jpeg_decode", "pil") == "device":           # MODEL.B200.JPEG_DECODE: one decode batch
+            from ...data.transforms import EncodedImage
+            encoded = []
+            for name in names:
+                with open(name, "rb") as f:
+                    encoded.append(EncodedImage(f.read()))
+            images = transform.decode_batch(encoded)
+        else:
+            images = (Image.open(name).convert("RGB") for name in names)
+        frames = []
+        for img in images:
+            img = transform(img)
             if isinstance(img, tuple):
                 img = img[0]
             frames.append(img.view(1, *img.shape))
