@@ -596,7 +596,7 @@ plain_softmax_kernel(float* __restrict__ s, __half* __restrict__ p16, int p_spli
   }
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
-  const float inv = 1.0f / sum;
+  const float inv = sum > 0.f ? 1.0f / sum : 0.f;   // no valid key (m_valid == 0): every probability 0, not 0 * inf
   if (p16 && p_split) {
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
@@ -748,11 +748,10 @@ static int relation_softmax_pe_impl(float* logits, void* probs_f16, int p_split,
   // with FFMAs; 3750 keys (two passes over 163 MB of fp32 logits in global memory: bandwidth-bound) 250 vs 242 us
   if (use_mma && ldm <= 1024) {
     relation_softmax_mma_kernel<true><<<n_rows, kRelThreads, smem, stream>>>(pw);
-  } else if (use_mma > 1) {
-    relation_softmax_mma_kernel<false><<<n_rows, kRelThreads, 0, stream>>>(pw);
+  } else if (ldm <= 1024) {
+    relation_softmax_pe_kernel<true><<<n_rows, kRelThreads, smem, stream>>>(pw);
   } else {
-    if (ldm <= 1024) relation_softmax_pe_kernel<true><<<n_rows, kRelThreads, smem, stream>>>(pw);
-    else relation_softmax_pe_kernel<false><<<n_rows, kRelThreads, 0, stream>>>(pw);
+    relation_softmax_pe_kernel<false><<<n_rows, kRelThreads, 0, stream>>>(pw);
   }
   MEGA_CUDA_CHECK(cudaGetLastError());
   return MEGA_OK;

@@ -270,12 +270,14 @@ def position_matrix(bbox, ref_bbox):
     return torch.stack([dx, dy, dw, dh], dim=2)
 
 
-def position_embedding(bbox, ref_bbox, feat_dim=64, wave_length=1000.0):
+def position_embedding(bbox, ref_bbox, feat_dim=64, wave_length=1000.0, dim_mat=None):
     """roi_box_feature_extractors.py:125-144 + :240-250 -> [feat_dim, N, M]
-    (channel = coord*16 + {sin: k, cos: 8 + k}, k = 0..7)."""
+    (channel = coord*16 + {sin: k, cos: 8 + k}, k = 0..7). dim_mat: the divisors as given (e.g. the fp32 values the
+    engine passes, on the boxes' device) instead of the ones computed here."""
     pm = position_matrix(bbox, ref_bbox)
-    feat_range = torch.arange(0, feat_dim / 8)
-    dim_mat = torch.full((len(feat_range),), wave_length).pow(8.0 / feat_dim * feat_range)
+    if dim_mat is None:
+        feat_range = torch.arange(0, feat_dim / 8)
+        dim_mat = torch.full((len(feat_range),), wave_length).pow(8.0 / feat_dim * feat_range)
     div = (pm.unsqueeze(3) * 100.0) / dim_mat.view(1, 1, 1, -1)
     emb = torch.cat([div.sin(), div.cos()], dim=3)                      # [N, M, 4, 16]
     emb = emb.reshape(emb.shape[0], emb.shape[1], -1)                   # [N, M, 64]
