@@ -284,6 +284,7 @@ int encode_conv_gemm_problem(const mega_conv_gemm_desc* d, CUtensorMap* tmA_p, C
   p.total_units = tiles * p.kb_per_tile;
   p.total_tiles = tiles;
   p.stream_k = d->stream_k ? 1 : 0;
+  p.n_fast = 0;
   p.seg_len = g_seg_len;
   p.b_lo_tap_off = d->b_lo_tap_off;
   p.res_split = d->res_split ? 1 : 0;
@@ -332,6 +333,11 @@ extern "C" int mega_conv_gemm(const mega_conv_gemm_desc* d, void* stream_v) {
   int ctas = 0;
   const int erc = encode_conv_gemm_problem(d, &tmA, &tmB, &tmOut, &tmRes, &p, &ctas);
   if (erc != MEGA_OK) return erc;
+  // 3xFP16 whole tiles run n-fastest: the CTAs of one wave then cover a few M tiles with all their N tiles, so each
+  // activation tile comes from HBM once and its other N tiles read it from L2. In m-fastest order, the next N tile reads
+  // the same A tile a wave later, and an A larger than L2 (res4 conv1, the res5 1x1 convs: 78 MB) comes from HBM once
+  // per N tile. Stream-K launches keep the m-fastest order, and with it their split points.
+  if (d->precision == kModeF16x3 && !p.stream_k && p.n_tiles > 1) p.n_fast = 1;
   const bool out16 = d->out_f16 != 0;
   dim3 grid(static_cast<unsigned>(ctas), 1, 1);
   const int pdl = d->pdl ? 1 : 0;

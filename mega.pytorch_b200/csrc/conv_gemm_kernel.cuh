@@ -93,6 +93,7 @@ struct ConvGemmParams {
   long long total_units;     // batch * m_tiles * n_tiles * kb_per_tile
   long long total_tiles;     // batch * m_tiles * n_tiles
   int stream_k;              // 1: k-block granular split across CTAs, 0: whole tiles round-robin
+  int n_fast;                // 3xFP16 whole-tile launches only: tiles ordered with the n-tile fastest (decode_tile)
   float* part_ws;            // [grid][2][128][BN] partial accumulators
   int* counters;             // [tiles], zero between launches
   int seg_len;               // 3xTF32 / 3xFP16: k-blocks accumulated by the tensor core before the RN fold into the master accumulator
@@ -132,12 +133,21 @@ struct TileCoord {
 
 // Work-list indices are 32-bit (the host checks total_units * grid < 2^31): 64-bit divisions cost hundreds of cycles
 // on the single-thread critical paths of the producer / MMA roles.
-__device__ __forceinline__ TileCoord decode_tile(const ConvGemmParams& p, int t, int bn) {
+// Tiles are ordered (batch, n-tile, m-tile) with m fastest, or, with n_fast, (batch, m-tile, n-tile) with n fastest.
+__device__ __forceinline__ TileCoord decode_tile(const ConvGemmParams& p, int t, int bn, bool n_fast = false) {
   TileCoord c;
-  const int m_tile = t % p.m_tiles;
-  const int rest = t / p.m_tiles;
-  const int n_tile = rest % p.n_tiles;
-  c.batch = rest / p.n_tiles;
+  int m_tile, n_tile;
+  if (n_fast) {
+    n_tile = t % p.n_tiles;
+    const int rest = t / p.n_tiles;
+    m_tile = rest % p.m_tiles;
+    c.batch = rest / p.m_tiles;
+  } else {
+    m_tile = t % p.m_tiles;
+    const int rest = t / p.m_tiles;
+    n_tile = rest % p.n_tiles;
+    c.batch = rest / p.n_tiles;
+  }
   const int tw_i = m_tile % p.tiles_w;
   const int th_i = (m_tile / p.tiles_w) % p.tiles_h;
   c.img = m_tile / (p.tiles_w * p.tiles_h);
@@ -737,7 +747,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       int kb0, kb1;
       const bool b_lo = SPLIT3 && p.b_lo_tap_off > 0;    // pre-split weights: the low parts come by TMA too
       while (it.next(t, kb0, kb1)) {
-        const TileCoord tc = decode_tile(p, t, BN);
+        const TileCoord tc = decode_tile(p, t, BN, PK && p.n_fast);
         for (int pass = 0; pass < (BN > pass_n(BN) ? 2 : 1); ++pass)
           produce_pass<STAGES>(&tmA, &tmB, full_bar, empty_bar, ps, smem, L::kStageBytes, L::kABytes,
                                b_lo ? L::kABytes + L::kBBytes : 0, kBK, L::kHalf + (b_lo ? L::kBBytes : 0), p, tc,
@@ -827,7 +837,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const bool res_split = p.res_split != 0;
     const float slope = p.relu == 2 ? 0.1f : 0.f;
     for (int tile_item = 0; it.next(t, kb0, kb1); ++tile_item) {
-      const TileCoord tc = decode_tile(p, t, BN);
+      const TileCoord tc = decode_tile(p, t, BN, p.n_fast);
       const bool complete = (kb0 == 0 && kb1 == KB);
       const StoreBox box = store_box(p, tc, q);
       const int nchunks = min(BN / 32, (p.cout - tc.n0 + 31) / 32);
@@ -844,7 +854,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       {   // the next tile's slice into [bsel ^ 1], which no warp reads before the next tile's barrier
         int t2;
         if (it.peek(t2) && epi_tid < BN) {
-          const TileCoord tc2 = decode_tile(p, t2, BN);
+          const TileCoord tc2 = decode_tile(p, t2, BN, p.n_fast);
           const int n = tc2.n0 + epi_tid;
           const bool valid = p.bias && n < p.cout;
           cp_async_f32(bias_s + (bsel ^ 1) * BN + epi_tid,
