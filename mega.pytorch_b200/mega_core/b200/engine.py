@@ -69,6 +69,9 @@ class EngineConfig:
     # MODEL.RPN_ONLY (single-frame, DFF and FGFA engines): the result is the RPN's proposals; the box head (res5, the
     # channel reduction, ROIAlign, fc6 / fc7, the predictor) is neither loaded nor run
     rpn_only = False
+    # MODEL.RESNETS.STRIDE_IN_1X1: which conv of res3 / res4's first bottleneck carries the stride, the 1x1 conv1 (True,
+    # the MSRA layout) or the 3x3 conv2 (False, the layout of the Caffe2 / fb.torch ResNe(X)t and torchvision weights)
+    stride_in_1x1 = True
 
     def __init__(self, **kw):
         for k, v in kw.items():
@@ -136,8 +139,13 @@ class _Block:
 class ResNetStages:
     """a sequence of bottleneck stages over NHWC activations (resnet.py:239-344)."""
 
-    def __init__(self, sd, prefix, layer_ids, dev, dilation=1, first_stride_of=None, dtype=torch.float32):
+    def __init__(self, sd, prefix, layer_ids, dev, dilation=1, first_stride_of=None, dtype=torch.float32,
+                 stride_in_1x1=True):
         self.dev, self.dtype = dev, dtype
+        # MODEL.RESNETS.STRIDE_IN_1X1 (resnet.py:272-275): True, the MSRA layout, strides a stage's first conv1;
+        # False (the fb.torch / Caffe2 ResNe(X)t and torchvision layout) strides its 3x3 conv2. The downsample 1x1 is
+        # strided in both, and the output sizes are the same: (H - 1) // 2 + 1 either way.
+        self.stride_in_1x1 = stride_in_1x1
         self.stages = []
         for li in layer_ids:
             blocks = []
@@ -228,13 +236,17 @@ class ResNetStages:
                 n, h, w, _ = x.shape
                 xs = x[:, ::2, ::2, :] if blk.stride == 2 else x
                 ho, wo = xs.shape[1], xs.shape[2]
-                t1 = self._buf("t1", (n, ho, wo, blk.mid))
+                x1 = xs if self.stride_in_1x1 else x         # conv1's input: strided view, or the full map
+                t1 = self._buf("t1", (n, x1.shape[1], x1.shape[2], blk.mid))
                 t2 = self._buf("t2", (n, ho, wo, blk.mid))
-                ops.conv_gemm(xs, blk.w1, t1, scale=blk.s1, bias=blk.b1, relu=True, max_ctas=max_ctas)
+                ops.conv_gemm(x1, blk.w1, t1, scale=blk.s1, bias=blk.b1, relu=True, max_ctas=max_ctas)
                 # a grouped conv2 goes in as its batched launch (the fields spelled out, not groups=: stand-ins for
                 # conv_gemm that know batched launches serve it unchanged)
+                kw2 = ops.grouped_fields(blk.w2) if blk.groups > 1 else {}
+                if x1 is not xs:
+                    kw2["stride"] = (2, 2)
                 ops.conv_gemm(t1, blk.w2, t2, taps=(3, 3), dil=blk.dil, pad=blk.dil, scale=blk.s2, bias=blk.b2,
-                              relu=True, max_ctas=max_ctas, **(ops.grouped_fields(blk.w2) if blk.groups > 1 else {}))
+                              relu=True, max_ctas=max_ctas, **kw2)
                 if blk.wd is not None:
                     idn = self._buf("idn", (n, ho, wo, blk.cout))
                     ops.conv_gemm(xs, blk.wd, idn, scale=blk.sd, bias=blk.bd, relu=False, max_ctas=max_ctas)
@@ -253,7 +265,7 @@ class ResNetStages:
 class Backbone:
     """ResNet C4 body: stem + res2..res4 (modeling/backbone/resnet.py:145-152, :347-366)."""
 
-    def __init__(self, sd, dev, prefix="backbone.body.", dtype=torch.float32):
+    def __init__(self, sd, dev, prefix="backbone.body.", dtype=torch.float32, stride_in_1x1=True):
         self.dev, self.dtype = dev, dtype
         w = sd[prefix + "stem.conv1.weight"].float().reshape(64, 147)
         wp = torch.zeros(1, 64, 160)
@@ -267,7 +279,7 @@ class Backbone:
         self.stem_wr = wr.contiguous().to(dev).to(dtype)
         self.stem_s, self.stem_b = fold_bn(sd, prefix + "stem.bn1.", dev)
         self.stages = ResNetStages(sd, prefix, (1, 2, 3), dev, first_stride_of=lambda li: 2 if li > 1 else 1,
-                                   dtype=dtype)
+                                   dtype=dtype, stride_in_1x1=stride_in_1x1)
         self._bufs = {}
         self._chains = {}
         self.out_channels = self.stages.stages[-1][-1].cout
@@ -395,7 +407,7 @@ class HeadCommon:
         ops.AUTOTUNE[0] = os.environ.get("MEGA_B200_AUTOTUNE", "1") != "0"
         ops.load_tuned(os.environ.get("MEGA_B200_TUNED", os.path.join(os.path.dirname(__file__), "tuned_b200.json")))
         self.act = act = cfg.act_dtype
-        self.backbone = Backbone(sd, dev, dtype=act)
+        self.backbone = Backbone(sd, dev, dtype=act, stride_in_1x1=cfg.stride_in_1x1)
         self.rpn_w = pack_conv(sd["rpn.head.conv.weight"], dev, act)
         self.rpn_b = sd["rpn.head.conv.bias"].float().contiguous().to(dev)
         a = sd["rpn.head.cls_logits.weight"].shape[0]

@@ -13,10 +13,11 @@ def build_detection_model(cfg):
     return _DETECTION_META_ARCHITECTURES[cfg.MODEL.META_ARCHITECTURE](cfg)
 
 
-def vid_config(method="mega", conv_body="R-101-C4", device="cuda", num_groups=1, width_per_group=64):
+def vid_config(method="mega", conv_body="R-101-C4", device="cuda", num_groups=1, width_per_group=64, stride_in_1x1=True):
     """the configuration tools/test_net.py ends up with for the VID configs: defaults <- BASE_RCNN_1gpu.yaml
     <- configs/MEGA/vid_R_101_C4_MEGA_1x.yaml (or configs/vid_R_50_C4_1x.yaml for method="base");
-    num_groups / width_per_group: MODEL.RESNETS.NUM_GROUPS / WIDTH_PER_GROUP (32 / 8 for a ResNeXt-101 32x8d body)"""
+    num_groups / width_per_group: MODEL.RESNETS.NUM_GROUPS / WIDTH_PER_GROUP (32 / 8 for a ResNeXt-101 32x8d body);
+    stride_in_1x1: MODEL.RESNETS.STRIDE_IN_1X1 (False for the Caffe2 / fb.torch ResNe(X)t and torchvision weights)"""
     from ...config import cfg as base
     c = base.clone()
     c.merge_from_dict({
@@ -24,7 +25,8 @@ def vid_config(method="mega", conv_body="R-101-C4", device="cuda", num_groups=1,
                   "RPN": {"ANCHOR_SIZES": (64, 128, 256, 512), "PRE_NMS_TOP_N_TEST": 6000, "POST_NMS_TOP_N_TEST": 300},
                   "ROI_HEADS": {"SCORE_THRESH": 0.001, "NMS": 0.5, "DETECTIONS_PER_IMG": 300},
                   "ROI_BOX_HEAD": {"NUM_CLASSES": 31, "POOLER_RESOLUTION": 7, "PREDICTOR": "FPNPredictor"},
-                  "RESNETS": {"RES5_DILATION": 2, "NUM_GROUPS": num_groups, "WIDTH_PER_GROUP": width_per_group},
+                  "RESNETS": {"RES5_DILATION": 2, "NUM_GROUPS": num_groups, "WIDTH_PER_GROUP": width_per_group,
+                              "STRIDE_IN_1X1": bool(stride_in_1x1)},
                   "BACKBONE": {"CONV_BODY": conv_body}},
         "INPUT": {"MIN_SIZE_TEST": 600, "MAX_SIZE_TEST": 1000}, "TEST": {"IMS_PER_BATCH": 1, "DETECTIONS_PER_IMG": 300}})
     if method == "mega":
@@ -51,9 +53,11 @@ def vid_config(method="mega", conv_body="R-101-C4", device="cuda", num_groups=1,
     return c
 
 
-def build_detection_model_from_state_dict(sd, method="mega", device="cuda", precision=None):
+def build_detection_model_from_state_dict(sd, method="mega", device="cuda", precision=None, stride_in_1x1=True):
     """convenience for benchmarks/tests: infer the conv body (depth, ResNeXt groups and width), REDUCE_CHANNEL, MEGA's
-    GLOBAL.RES_STAGE and RDN's ADVANCED_STAGE from the state dict, build, load, eval"""
+    GLOBAL.RES_STAGE and RDN's ADVANCED_STAGE from the state dict, build, load, eval. stride_in_1x1
+    (MODEL.RESNETS.STRIDE_IN_1X1) is given by the caller: both stride layouts have the same keys and shapes, so the
+    weights cannot tell which one they were trained with"""
     fe = "roi_heads.box.feature_extractor."
     n3 = 0
     while ("backbone.body.layer3.%d.conv1.weight" % n3) in sd:
@@ -61,7 +65,7 @@ def build_detection_model_from_state_dict(sd, method="mega", device="cuda", prec
     body = {6: "R-50-C4", 23: "R-101-C4"}.get(n3)
     w2 = sd["backbone.body.layer1.0.conv2.weight"]              # [G * width, width, 3, 3]
     cfg = vid_config(method, body or "R-101-C4", device, num_groups=w2.shape[0] // w2.shape[1],
-                     width_per_group=w2.shape[1])
+                     width_per_group=w2.shape[1], stride_in_1x1=stride_in_1x1)
     if precision is not None:
         cfg.MODEL.B200.PRECISION = precision
     cfg.MODEL.VID.ROI_BOX_HEAD.REDUCE_CHANNEL = (fe + "conv.weight") in sd

@@ -48,23 +48,27 @@ def _image_size(images):
 
 
 class Bottleneck(nn.Module):
-    def __init__(self, cin, mid, cout, stride, dilation, groups=1):
+    def __init__(self, cin, mid, cout, stride, dilation, groups=1, stride_in_1x1=True):
         super().__init__()
         if cin != cout:
             self.downsample = nn.Sequential(Conv2d(cin, cout, 1, stride=(stride if dilation == 1 else 1), bias=False),
                                             FrozenBatchNorm2d(cout))
-        self.conv1 = Conv2d(cin, mid, 1, stride=(1 if dilation > 1 else stride), bias=False)
+        if dilation > 1:
+            stride = 1
+        s1, s3 = (stride, 1) if stride_in_1x1 else (1, stride)          # resnet.py:272-275
+        self.conv1 = Conv2d(cin, mid, 1, stride=s1, bias=False)
         self.bn1 = FrozenBatchNorm2d(mid)
-        self.conv2 = Conv2d(mid, mid, 3, padding=dilation, dilation=dilation, groups=groups, bias=False)
+        self.conv2 = Conv2d(mid, mid, 3, stride=s3, padding=dilation, dilation=dilation, groups=groups, bias=False)
         self.bn2 = FrozenBatchNorm2d(mid)
         self.conv3 = Conv2d(mid, cout, 1, bias=False)
         self.bn3 = FrozenBatchNorm2d(cout)
 
 
-def _stage(cin, mid, cout, n, stride, dilation=1, groups=1):
+def _stage(cin, mid, cout, n, stride, dilation=1, groups=1, stride_in_1x1=True):
     blocks = []
     for i in range(n):
-        blocks.append(Bottleneck(cin if i == 0 else cout, mid, cout, stride if i == 0 else 1, dilation, groups))
+        blocks.append(Bottleneck(cin if i == 0 else cout, mid, cout, stride if i == 0 else 1, dilation, groups,
+                                 stride_in_1x1))
     return nn.Sequential(*blocks)
 
 
@@ -87,11 +91,11 @@ class ResNetBody(nn.Module):
     def __init__(self, cfg):
         super().__init__()
         b = BLOCKS[cfg.MODEL.BACKBONE.CONV_BODY]
-        g = cfg.MODEL.RESNETS.NUM_GROUPS
+        g, s1x1 = cfg.MODEL.RESNETS.NUM_GROUPS, cfg.MODEL.RESNETS.STRIDE_IN_1X1
         self.stem = Stem()
-        self.layer1 = _stage(64, bottleneck_width(cfg, 1), 256, b[0], 1, groups=g)
-        self.layer2 = _stage(256, bottleneck_width(cfg, 2), 512, b[1], 2, groups=g)
-        self.layer3 = _stage(512, bottleneck_width(cfg, 3), 1024, b[2], 2, groups=g)
+        self.layer1 = _stage(64, bottleneck_width(cfg, 1), 256, b[0], 1, groups=g, stride_in_1x1=s1x1)
+        self.layer2 = _stage(256, bottleneck_width(cfg, 2), 512, b[1], 2, groups=g, stride_in_1x1=s1x1)
+        self.layer3 = _stage(512, bottleneck_width(cfg, 3), 1024, b[2], 2, groups=g, stride_in_1x1=s1x1)
         self.out_channels = 1024
 
 
@@ -373,8 +377,6 @@ def engine_config_from(cfg):
     v = m.VID
     win = {"rdn": v.RDN, "fgfa": v.FGFA}.get(v.METHOD, v.MEGA)     # window geometry of the method
     unsupported = []
-    if not m.RESNETS.STRIDE_IN_1X1:
-        unsupported.append("MODEL.RESNETS.STRIDE_IN_1X1 = False (the engines put the stride on the 1x1 conv, resnet.py:288-291)")
     if v.METHOD in ("rdn", "mega") and v.RPN.REF_PRE_NMS_TOP_N != m.RPN.PRE_NMS_TOP_N_TEST:
         unsupported.append("MODEL.VID.RPN.REF_PRE_NMS_TOP_N != MODEL.RPN.PRE_NMS_TOP_N_TEST (the reference proposals of a frame "
                            "are taken as the prefix of its key proposals, which needs equal pre-NMS sets)")
@@ -435,4 +437,5 @@ def engine_config_from(cfg):
         aspect_ratios=tuple(m.RPN.ASPECT_RATIOS), anchor_stride=m.RPN.ANCHOR_STRIDE[0],
         num_classes=m.ROI_BOX_HEAD.NUM_CLASSES,
         precision=os.environ.get("MEGA_B200_PRECISION", m.B200.PRECISION if "B200" in m else "f16"),
-        **({"rpn_only": True} if m.RPN_ONLY else {}))
+        **({"rpn_only": True} if m.RPN_ONLY else {}),
+        **({} if m.RESNETS.STRIDE_IN_1X1 else {"stride_in_1x1": False}))

@@ -3,6 +3,7 @@ bench.py launch, so that tile choices -- hence summation orders, hence parity nu
     python tools/tune_all.py            -> gpurun_out/tuned_b200.json  (copy to mega.pytorch_b200/mega_core/b200/)
 Runs the GPU test-suite in-process (its engines autotune every new shape), then the benchmark configurations
 (MEGA R-101 at 600x1000 in f16 and fp32x3 with 1 / 2 / 4 key frames per step, tf32; the frame-parallel row splits;
+MEGA R-101 / X-101 with 3x3-strided bottlenecks;
 RDN / FGFA), and dumps the union."""
 import os
 import sys
@@ -43,6 +44,20 @@ with torch.no_grad():
         del eng
         torch.cuda.empty_cache()
         ops.save_tuned(out)
+    # MODEL.RESNETS.STRIDE_IN_1X1 False, dense and X-101 32x8d: the full-resolution conv1 and the 3x3 / stride-2 conv2 of
+    # res3 / res4's first blocks (150x250 -> 75x125, 75x125 -> 38x63)
+    for arch in ("mega_r101", "mega_x101"):
+        sdx = synth.make_state_dict(arch, seed=0)
+        for prec in ("f16", "fp32x3"):
+            eng = engine.MegaEngine(sdx, engine.EngineConfig(precision=prec, stride_in_1x1=False), device=dev)
+            eng.start_video(frames[0], frames[1:13], [frames[(3 * j + 1) % 16] for j in range(10)], w, h)
+            eng.step_batched(pairs[0], w, h)
+            eng.stepn_batched(torch.cat([pairs[j] for j in range(4)], 0), w, h)
+            torch.cuda.synchronize()
+            print(arch, prec, "stride_in_1x1 False: entries", len(ops.TUNED), flush=True)
+            del eng
+            torch.cuda.empty_cache()
+            ops.save_tuned(out)
     for arch, cls, kw in (("rdn_r101", engine.RdnEngine, dict(all_frame_interval=37, key_frame_location=18, stage=2, advanced_stage=1)),
                           ("fgfa_r101", engine.FgfaEngine, dict(all_frame_interval=19, key_frame_location=9))):
         sdx = synth.make_state_dict(arch, seed=4)
