@@ -517,6 +517,45 @@ int mega_proposal_recall(const float* prop_boxes, const float* prop_scores, cons
                          int limit, float iou_thresh, void* workspace, long long workspace_bytes, float* gt_overlaps,
                          unsigned long long* stats, void* stream);
 
+/* ------------------------------------------------------- detection AP of a whole dataset (VID evaluation)
+ * calc_detection_vid_prec_rec and the curve half of calc_detection_vid_ap of the reference
+ * (data/datasets/evaluation/vid/vid_eval.py:156-343) for a whole dataset and num_ranges motion ranges in one sequence
+ * of launches; replaces the per-image / per-class Python loop of :185-284 that the reference runs once per range.
+ * Input (device memory unless noted), flattened per image i in [0, num_images):
+ *   detections [det_offsets[i], det_offsets[i+1]) of det_boxes [num_dets, 4] xyxy fp32 (16-byte aligned), det_scores,
+ *   det_labels int32 in [0, num_classes); det_scale [num_images, 2] fp32 (8-byte aligned): the box of image i is
+ *   (x1 * sw, y1 * sh, x2 * sw, y2 * sh) in fp32 -- BoxList.resize to the image's original size, sw = (float)(w / w_pred);
+ *   ground truth [gt_offsets[i], gt_offsets[i+1]) of gt_boxes [num_gt, 4], gt_labels int32, gt_motion fp64 (the GT's
+ *   motion IoU; NaN for a GT without one: never ignored);
+ *   ranges (HOST memory) [num_ranges, 3] fp64: lo, hi, empty_weight of each range (a GT is ignored iff motion < lo or
+ *   motion > hi; empty_weight as the host evaluator computes it, 0 where the fraction is 1);
+ *   step_offsets [num_classes + 1] int64, ascending, step_offsets[num_classes] = num_steps: the capacity of class c's
+ *   recall steps is step_offsets[c+1] - step_offsets[c]; the number of GT of class c plus 2 always suffices.
+ * Order ("stable ties"): per image and class the detections by score, descending, ties later index first
+ * (argsort(kind="stable")[::-1]); per class the per-image lists concatenated in image order and ordered again the same
+ * way (ties: later image first, then lower index). Per (image, class, range): the greedy matching of
+ * mega_vid_match_host. Per (class, range), in the class order: tp = cumulative count of matched non-ignored
+ * detections, fp = cumulative fp64 sum (left to right) of the ignore weights of the unmatched ones (1 for weight 0),
+ * prec = tp / (fp + tp + 2^-52), rec = tp / n_pos.
+ * Output: prec, rec [num_ranges, num_dets] fp64, class c at positions [begin_c, end_c) of each range; stats int64
+ * [3 C + 2 R C + 1] (C = num_classes, R = num_ranges): present[C] (1: the class occurs in a detection or GT), begin[C],
+ * end[C], n_pos[R][C], n_steps[R][C], rejected. steps [R, 3, num_steps] fp64: for (r, c) with n_pos > 0, n_steps[r][c]
+ * points at step_offsets[c] of each of the three rows -- mrec[i+1] - mrec[i], mpre[i+1], mrec[i+1] at every i with
+ * mrec[i+1] != mrec[i] (mrec = [0, rec, 1], mpre = [0, prec, 0] made non-increasing from the right), in increasing i:
+ * the AP is np.sum(row0 * row1); n_steps = -1 where n_pos = 0 or the class is absent. rejected counts labels out of
+ * range and classes whose steps exceed their capacity (a correct call gives 0).
+ * Deterministic; no allocation, no synchronisation, everything on `stream`. workspace: >=
+ * mega_vid_eval_workspace_bytes(...) bytes, 256-byte aligned; -1 for arguments out of range (num_ranges in [1, 8],
+ * num_dets < 2^31, ceil(log2 num_images) + ceil(log2 num_classes) <= 32). */
+long long mega_vid_eval_workspace_bytes(long long num_dets, long long num_gt, int num_images, int num_classes,
+                                        int num_ranges);
+int mega_vid_eval(const float* det_boxes, const float* det_scores, const int* det_labels, const long long* det_offsets,
+                  const float* det_scale, long long num_dets, const float* gt_boxes, const int* gt_labels,
+                  const double* gt_motion, const long long* gt_offsets, long long num_gt, int num_images,
+                  int num_classes, const double* ranges, int num_ranges, float iou_thresh,
+                  const long long* step_offsets, long long num_steps, void* workspace, long long workspace_bytes,
+                  double* prec, double* rec, long long* stats, double* steps, void* stream);
+
 /* ------------------------------------------------------------- baseline JPEG decode (SURVEY.md section 8f row 1)
  * Replaces `PIL.Image.open(path).convert("RGB")` of the reference's datasets (data/datasets/vid.py:95 and the frames
  * the detectors open themselves) with the SAME uint8 pixels, produced on the device: libjpeg's defaults as Pillow

@@ -242,6 +242,11 @@ lib.mega_proposal_recall_workspace_bytes.argtypes = [_i, _i, _i, _i]
 lib.mega_proposal_recall_workspace_bytes.restype = _ll
 lib.mega_proposal_recall.argtypes = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _ll, _vp, _vp, _vp]
 lib.mega_proposal_recall.restype = _i
+lib.mega_vid_eval_workspace_bytes.argtypes = [_ll, _ll, _i, _i, _i]
+lib.mega_vid_eval_workspace_bytes.restype = _ll
+lib.mega_vid_eval.argtypes = [_vp, _vp, _vp, _vp, _vp, _ll, _vp, _vp, _vp, _vp, _ll, _i, _i, _vp, _i, _f, _vp, _ll, _vp,
+                              _ll, _vp, _vp, _vp, _vp, _vp]
+lib.mega_vid_eval.restype = _i
 
 
 class JpegInfo(ctypes.Structure):
@@ -287,5 +292,6 @@ EXPORTS = [
     "mega_seq_nms_workspace_bytes", "mega_seq_nms",
     "mega_image_transform_u8_ex", "mega_bbox_aug_workspace_bytes", "mega_bbox_aug_collect", "mega_bbox_aug_merge",
     "mega_proposal_recall_workspace_bytes", "mega_proposal_recall",
+    "mega_vid_eval_workspace_bytes", "mega_vid_eval",
     "mega_jpeg_probe", "mega_jpeg_entropy_decode", "mega_jpeg_plan_batch", "mega_jpeg_decode_batch",
 ]

@@ -1050,6 +1050,37 @@ def proposal_recall(prop_boxes, prop_scores, prop_offsets, gt_boxes, gt_offsets,
     LAUNCHES[0] += 1
 
 
+def vid_eval_workspace_bytes(num_dets, num_gt, num_images, num_classes, num_ranges):
+    nbytes = lib.mega_vid_eval_workspace_bytes(num_dets, num_gt, num_images, num_classes, num_ranges)
+    if nbytes < 0:
+        raise _lib.MegaError("vid_eval: %d detections, %d GT, %d images, %d classes, %d ranges: out of range (1..8 "
+                             "ranges, < 2^31 detections, ceil(log2 images) + ceil(log2 classes) <= 32)" % (
+                                 num_dets, num_gt, num_images, num_classes, num_ranges))
+    return nbytes
+
+
+def vid_eval(det_boxes, det_scores, det_labels, det_offsets, det_scale, gt_boxes, gt_labels, gt_motion, gt_offsets,
+             num_classes, ranges, iou_thresh, step_offsets, num_steps, prec, rec, stats, steps):
+    """detection AP curves of a dataset for every motion range (include/mega_b200.h, mega_vid_eval). det_boxes [P, 4]
+    fp32, det_scores [P], det_labels [P] int32, det_offsets [N + 1] int64, det_scale [N, 2] fp32, gt_boxes [G, 4],
+    gt_labels [G] int32, gt_motion [G] fp64, gt_offsets [N + 1], step_offsets [C + 1] int64 (device); ranges: host
+    list of (lo, hi, empty_weight). Outputs prec / rec [R, P] fp64, stats int64, steps [R, 3, num_steps] fp64. The
+    workspace is allocated for this call only. No synchronisation."""
+    require_cuda(det_boxes, det_scores, det_labels, det_offsets, det_scale, gt_boxes, gt_labels, gt_motion, gt_offsets,
+                 step_offsets, prec, rec, stats, steps)
+    n = det_offsets.numel() - 1
+    p, g, r = det_scores.numel(), gt_labels.numel(), len(ranges)
+    nbytes = vid_eval_workspace_bytes(p, g, n, num_classes, r)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=stats.device)
+    host_ranges = (ctypes.c_double * (3 * r))(*[float(v) for rng in ranges for v in rng])
+    check(lib.mega_vid_eval(ptr(det_boxes), ptr(det_scores), ptr(det_labels), ptr(det_offsets), ptr(det_scale), p,
+                            ptr(gt_boxes), ptr(gt_labels), ptr(gt_motion), ptr(gt_offsets), g, n, int(num_classes),
+                            ctypes.cast(host_ranges, ctypes.c_void_p), r, float(iou_thresh), ptr(step_offsets),
+                            int(num_steps), ptr(ws), nbytes, ptr(prec), ptr(rec), ptr(stats), ptr(steps), stream_ptr()),
+          "mega_vid_eval")
+    LAUNCHES[0] += 9
+
+
 # --------------------------------------------------------------------------- FGFA helpers (csrc/fgfa.cu)
 def _is16(t):
     return 1 if t.dtype == torch.float16 else 0

@@ -135,7 +135,11 @@ _C = CfgNode({
         # decodes all frames of an item as one batch (mega_core.data.transforms.decode_jpeg_exact: Huffman decoding on
         # host threads, IDCT / upsampling / colour conversion in CUDA, PIL's pixels bit for bit). TEST.BBOX_AUG keeps
         # PIL either way: its collator hands PIL images to im_detect_bbox_aug, which transforms each pass itself
-        "B200": {"PRECISION": "f16", "JPEG_DECODE": "pil",
+        # VID_EVAL (B200 build only): "host" -- detection AP by the host evaluator, per image and class, once per
+        # motion range, ties between equal scores in numpy's default sort order, as the reference; "device" -- all
+        # motion ranges of the dataset in one pass of the GPU evaluator (csrc/vid_eval.cu), ties in a fixed order
+        # (argsort(kind="stable")[::-1]), equal to the host evaluator with stable_ties=True bit for bit
+        "B200": {"PRECISION": "f16", "JPEG_DECODE": "pil", "VID_EVAL": "host",
                  "SEQ_NMS": {"ENABLED": False, "LINK_IOU": 0.5, "NMS_IOU": 0.3, "RESCORE": "avg"}},
     },
     "INPUT": {"MIN_SIZE_TRAIN": (800,), "MAX_SIZE_TRAIN": 1333, "MIN_SIZE_TEST": 800, "MAX_SIZE_TEST": 1333,

@@ -126,14 +126,16 @@ def inference(cfg, model, data_loader, dataset_name, iou_types=("bbox",), motion
         torch.save(predictions, os.path.join(output_folder, "predictions.pth"))
     return vid_evaluation(dataset=dataset, predictions=predictions, output_folder=output_folder, box_only=box_only,
                           motion_specific=motion_specific, iou_types=iou_types, expected_results=expected_results,
-                          expected_results_sigma_tol=expected_results_sigma_tol)
+                          expected_results_sigma_tol=expected_results_sigma_tol,
+                          vid_eval=str(getattr(getattr(cfg.MODEL, "B200", None), "VID_EVAL", "host")))
 
 
 def inference_no_model(data_loader, iou_types=("bbox",), motion_specific=False, box_only=False, expected_results=(),
-                       expected_results_sigma_tol=4, output_folder=None, seq_nms=None):
+                       expected_results_sigma_tol=4, output_folder=None, seq_nms=None, vid_eval="host"):
     """engine/inference.py:137-160: score the predictions.pth of an earlier run. `seq_nms`: a dict with the keys of
     MODEL.B200.SEQ_NMS (ENABLED, LINK_IOU, NMS_IOU, RESCORE), e.g. dict(cfg.MODEL.B200.SEQ_NMS), to rescore the saved
-    predictions with Seq-NMS first (the file is not changed)"""
+    predictions with Seq-NMS first (the file is not changed). `vid_eval`: MODEL.B200.VID_EVAL, "host" or "device"
+    (all motion ranges in one pass of the GPU evaluator)"""
     predictions = torch.load(os.path.join(output_folder, "predictions.pth"), weights_only=False)
     seq = _seq_nms_kwargs(seq_nms)
     if seq is not None:
@@ -141,4 +143,4 @@ def inference_no_model(data_loader, iou_types=("bbox",), motion_specific=False, 
                                logging.getLogger("mega_core.inference"))
         predictions = [by_id[i] for i in range(len(predictions))]
     return vid_evaluation(dataset=data_loader.dataset, predictions=predictions, output_folder=output_folder,
-                          box_only=box_only, motion_specific=motion_specific)
+                          box_only=box_only, motion_specific=motion_specific, vid_eval=vid_eval)
