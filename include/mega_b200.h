@@ -356,6 +356,24 @@ int mega_deform_im2col(const float* input, const float* offset, const float* mas
                        int width, int kh, int kw, int pad_h, int pad_w, int stride_h, int stride_w, int dil_h, int dil_w,
                        int deformable_group, int kpad, float* cols, void* stream);
 
+/* ---------------------------- deformable bottleneck conv2 (MODEL.RESNETS.STAGE_WITH_DCN), NHWC sampling
+ * The middle launch of a deformable 3x3 conv (padding = dilation, one deformable group) between its offset conv and
+ * its contraction, both mega_conv_gemm launches. input [batch, height, width, channels] NHWC in `format`;
+ * offset [batch, Ho, Wo, offset_ld] fp32: channels 2 tap / 2 tap + 1 the (dh, dw) of tap = 3 i + j, and for
+ * modulated != 0 (DCN v2) channel 18 + tap the mask logit, whose sigmoid multiplies the sample. Output cols
+ * [batch, Ho, Wo, 9 * channels] in `format`, tap-major rows: cols[p][tap * channels + c] -- the A operand of a 1x1
+ * mega_conv_gemm with K = 9 * channels against the weight packed as [1, Cout, 9 * Cin] in the same order.
+ * Ho = (height - 1) / stride + 1, likewise Wo. The interpolation is the reference's deformable_im2col_bilinear in
+ * fp32 (csrc/cuda/deform_conv_kernel_cuda.cu:92-120, :475-504, :578-640) for every format; split-fp16 output is
+ * split as mega_split16_pack splits. channels % 32 == 0; input and cols 16-byte aligned. No allocation, no
+ * synchronisation, everything on `stream` (CUDA-graph capturable). */
+#define MEGA_DCN_FP32 0
+#define MEGA_DCN_FP16 1
+#define MEGA_DCN_SPLIT16 2
+int mega_dcn_sample_nhwc(const void* input, int format, int batch, int height, int width, int channels,
+                         const float* offset, int offset_ld, int modulated, int stride, int dil, void* cols,
+                         void* stream);
+
 /* ------------------- deformable position-sensitive ROI pooling forward (csrc/deform_pool.h:11-37) */
 int mega_deform_psroi_pooling_forward(const float* input, const float* rois, const float* trans, int num_rois,
                                       int channels, int height, int width, int no_trans, float spatial_scale,

@@ -5,10 +5,12 @@
 //     follows (`addmm_` per group in deform_conv_cuda.cu:228-243, :545-567) runs on the wgmma GEMM,
 //     so the column matrix is written K-major per output pixel: cols[b][h*Wo+w][c*kh*kw + i*kw + j];
 //   * deformable position-sensitive ROI pooling forward (csrc/cuda/deform_pool_kernel_cuda.cu:31-142).
-// None of them is reachable from the VID configs (STAGE_WITH_DCN all False, defaults.py:287; focal loss is
-// RetinaNet-only); they complete the `_C` operator surface.
+// They complete the `_C` operator surface (focal loss is RetinaNet-only). The engines' deformable backbone stages
+// (MODEL.RESNETS.STAGE_WITH_DCN) do not run through mega_deform_im2col: they sample NHWC activations into a tap-major
+// column operand (dcn_sample.cu); the tile kernel below shares its sample geometry with that kernel (dcn_sample.cuh).
 #include <float.h>
 #include "common.cuh"
+#include "dcn_sample.cuh"
 #include "mega_b200.h"
 
 namespace mega {
@@ -112,11 +114,6 @@ constexpr int kDcnPix = 32;
 constexpr int kDcnCh = 16;
 constexpr int kDcnMaxTaps = 49;     // up to 7x7 kernels in shared memory; larger ones take the scalar kernel
 
-struct DcnTap {          // geometry of one (tap, pixel) sample
-  int i00, i01, i10, i11;
-  float w00, w01, w10, w11;
-};
-
 __global__ void __launch_bounds__(128)
 deform_im2col_tile_kernel(const float* __restrict__ im, const float* __restrict__ offset, const float* __restrict__ mask,
                           int channels, int height, int width, int kh, int kw, int pad_h, int pad_w, int stride_h,
@@ -151,19 +148,7 @@ deform_im2col_tile_kernel(const float* __restrict__ im, const float* __restrict_
       const long long o = (static_cast<long long>(2 * tap) * ho + h_col) * wo + w_col;
       const float h_im = h_col * stride_h - pad_h + i * dil_h + __ldg(off + o);
       const float w_im = w_col * stride_w - pad_w + j * dil_w + __ldg(off + o + static_cast<long long>(ho) * wo);
-      if (h_im > -1 && w_im > -1 && h_im < height && w_im < width) {
-        const int h_low = static_cast<int>(floorf(h_im)), w_low = static_cast<int>(floorf(w_im));
-        const int h_high = h_low + 1, w_high = w_low + 1;
-        const float lh = h_im - h_low, lw = w_im - w_low, hh = 1.f - lh, hw = 1.f - lw;
-        const bool t0 = h_low >= 0, t1 = h_high <= height - 1, l0 = w_low >= 0, l1 = w_high <= width - 1;
-        g.i00 = (t0 && l0) ? h_low * width + w_low : -1;
-        g.i01 = (t0 && l1) ? h_low * width + w_high : -1;
-        g.i10 = (t1 && l0) ? h_high * width + w_low : -1;
-        g.i11 = (t1 && l1) ? h_high * width + w_high : -1;
-        g.w00 = hh * hw; g.w01 = hh * lw; g.w10 = lh * hw; g.w11 = lh * lw;
-      } else {
-        g.i00 = g.i01 = g.i10 = g.i11 = -2;     // the whole sample is outside: value 0
-      }
+      g = dcn_tap_geometry(h_im, w_im, height, width);
       // the modulation scalar of DCN v2 multiplies the interpolated value (kept as a separate factor, like the reference)
       if (msk) mvals[tap * kDcnPix + lane] = __ldg(msk + (static_cast<long long>(tap) * ho + h_col) * wo + w_col);
     }
@@ -178,7 +163,7 @@ deform_im2col_tile_kernel(const float* __restrict__ im, const float* __restrict_
   constexpr int kDcnUnroll = 8;
   for (int tap = warp; tap < taps; tap += 4) {
     const DcnTap g = geo[tap * kDcnPix + lane];
-    const bool inside = live && g.i00 != -2;
+    const bool inside = live && g.i00 != kDcnOutside;
     const float mval = (msk && live) ? mvals[tap * kDcnPix + lane] : 1.f;
     const float* plane0 = im + (static_cast<long long>(b) * channels + c0) * plane_sz;
     for (int cl0 = 0; cl0 < nch; cl0 += kDcnUnroll) {

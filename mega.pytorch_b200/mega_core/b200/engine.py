@@ -17,6 +17,7 @@ same arithmetic, see DESIGN.md):
 """
 import math
 import os
+import sys
 from collections import deque
 
 import numpy as np
@@ -128,6 +129,10 @@ def pack_conv(w, dev, dtype=torch.float32):
     return w.float().permute(2, 3, 0, 1).reshape(kh * kw, co, ci).contiguous().to(dev).to(dtype)
 
 
+# output rows of a deformable conv2's offset conv: its 18 (DCN v1) or 27 (v2) channels zero-padded to the narrowest N tile
+DCN_OFFSET_ROWS = 32
+
+
 # BaseStem.conv1 as a row-slab implicit GEMM over the bordered NHWC8 image (True) or through an im2col buffer (False)
 STEM_ROW_SLABS = [True]
 
@@ -155,10 +160,14 @@ class ResNetStages:
                 blk = _Block()
                 blk.w1 = pack_conv(sd[p + "conv1.weight"], dev, dtype)
                 blk.s1, blk.b1 = fold_bn(sd, p + "bn1.", dev)
-                w2 = sd[p + "conv2.weight"]
+                blk.dcn = (p + "conv2.conv.weight") in sd          # MODEL.RESNETS.STAGE_WITH_DCN: conv2 is a DFConv2d
+                w2 = sd[p + ("conv2.conv.weight" if blk.dcn else "conv2.weight")]
                 blk.groups = sd[p + "conv1.weight"].shape[0] // w2.shape[1]     # ResNeXt: conv2 is grouped
-                blk.w2 = (pack_conv(w2, dev, dtype) if blk.groups == 1
-                          else ops.pack_grouped_conv(w2.float(), blk.groups, dev, dtype))
+                if blk.dcn:
+                    self._init_dcn(blk, sd, p, w2, dev, dtype)
+                else:
+                    blk.w2 = (pack_conv(w2, dev, dtype) if blk.groups == 1
+                              else ops.pack_grouped_conv(w2.float(), blk.groups, dev, dtype))
                 blk.s2, blk.b2 = fold_bn(sd, p + "bn2.", dev)
                 blk.w3 = pack_conv(sd[p + "conv3.weight"], dev, dtype)
                 blk.s3, blk.b3 = fold_bn(sd, p + "bn3.", dev)
@@ -177,25 +186,48 @@ class ResNetStages:
         self._bufs = {}
         self.lane = 0       # interleaved chains (ops.chain(interleave=True)): each lane owns its scratch buffers
         self.split16 = False    # strict mode: weights and activations in the split-fp16 format (use_split16())
+        self.has_dcn = any(blk.dcn for blocks in self.stages for blk in blocks)
+        # runs each deformable sampling launch; Backbone.forward replaces it to cut its chain into segments there
+        self.cut = _run_now
+
+    @staticmethod
+    def _init_dcn(blk, sd, p, w, dev, dtype):
+        """DFConv2d (layers/misc.py:114-189) with one deformable group: conv2.offset, a 3x3 conv with bias whose 18 (v1)
+        or 27 (v2, modulated) output channels are zero-padded to DCN_OFFSET_ROWS; conv2.conv, the deformable conv, packed
+        [1, Cout, 9 Cin] tap-major for the contraction over the sampled columns (K = 9 Cin)"""
+        wo, bo = sd[p + "conv2.offset.weight"].float(), sd[p + "conv2.offset.bias"].float()
+        k, ci = wo.shape[0], wo.shape[1]
+        assert blk.groups == 1 and k in (18, 27) and tuple(wo.shape[2:]) == (3, 3), \
+            "%sconv2: deformable conv2 is served dense, with one deformable group (offset channels %d)" % (p, k)
+        blk.modulated = k == 27
+        wpad = torch.zeros(DCN_OFFSET_ROWS, ci, 3, 3)
+        wpad[:k] = wo
+        blk.wo = pack_conv(wpad, dev, dtype)
+        bpad = torch.zeros(DCN_OFFSET_ROWS)
+        bpad[:k] = bo
+        blk.bo = bpad.to(dev)
+        co = w.shape[0]
+        blk.w2 = w.float().permute(0, 2, 3, 1).reshape(1, co, 9 * ci).contiguous().to(dev).to(dtype)
 
     def use_split16(self):
         """strict mode ("3xFP16", ops.pack_weights_split16): every weight is packed once, every scratch buffer holds
         split-fp16 activations; forward() packs an fp32 input on entry and writes `out` in the format `out` is marked with"""
         for blocks in self.stages:
             for blk in blocks:
-                for name, sname in (("w1", "s1"), ("w2", "s2"), ("w3", "s3"), ("wd", "sd")):
+                for name, sname in (("w1", "s1"), ("w2", "s2"), ("w3", "s3"), ("wd", "sd"), ("wo", "so")):
                     if getattr(blk, name, None) is not None:     # the FrozenBatchNorm scale goes into the packed weights
-                        setattr(blk, name, ops.pack_weights_split16(getattr(blk, name), scale=getattr(blk, sname)))
+                        setattr(blk, name, ops.pack_weights_split16(getattr(blk, name), scale=getattr(blk, sname, None)))
                         setattr(blk, sname, None)
         self.split16 = True
         self._bufs = {}
 
-    def _buf(self, tag, shape):
+    def _buf(self, tag, shape, fp32=False):
+        """scratch activations in the engine's format; fp32=True: a plain fp32 buffer (the deformable offsets)"""
         key = (tag, tuple(shape), self.lane)
         t = self._bufs.get(key)
         if t is None:
-            t = torch.zeros(*shape, device=self.dev, dtype=self.dtype)
-            if self.split16:
+            t = torch.zeros(*shape, device=self.dev, dtype=torch.float32 if fp32 else self.dtype)
+            if self.split16 and not fp32:
                 ops.mark_split16(t)
             self._bufs[key] = t
         return t
@@ -240,13 +272,16 @@ class ResNetStages:
                 t1 = self._buf("t1", (n, x1.shape[1], x1.shape[2], blk.mid))
                 t2 = self._buf("t2", (n, ho, wo, blk.mid))
                 ops.conv_gemm(x1, blk.w1, t1, scale=blk.s1, bias=blk.b1, relu=True, max_ctas=max_ctas)
-                # a grouped conv2 goes in as its batched launch (the fields spelled out, not groups=: stand-ins for
-                # conv_gemm that know batched launches serve it unchanged)
-                kw2 = ops.grouped_fields(blk.w2) if blk.groups > 1 else {}
-                if x1 is not xs:
-                    kw2["stride"] = (2, 2)
-                ops.conv_gemm(t1, blk.w2, t2, taps=(3, 3), dil=blk.dil, pad=blk.dil, scale=blk.s2, bias=blk.b2,
-                              relu=True, max_ctas=max_ctas, **kw2)
+                if blk.dcn:
+                    self._dcn_conv2(blk, t1, t2, 2 if x1 is not xs else 1, max_ctas)
+                else:
+                    # a grouped conv2 goes in as its batched launch (the fields spelled out, not groups=: stand-ins for
+                    # conv_gemm that know batched launches serve it unchanged)
+                    kw2 = ops.grouped_fields(blk.w2) if blk.groups > 1 else {}
+                    if x1 is not xs:
+                        kw2["stride"] = (2, 2)
+                    ops.conv_gemm(t1, blk.w2, t2, taps=(3, 3), dil=blk.dil, pad=blk.dil, scale=blk.s2, bias=blk.b2,
+                                  relu=True, max_ctas=max_ctas, **kw2)
                 if blk.wd is not None:
                     idn = self._buf("idn", (n, ho, wo, blk.cout))
                     ops.conv_gemm(xs, blk.wd, idn, scale=blk.sd, bias=blk.bd, relu=False, max_ctas=max_ctas)
@@ -260,6 +295,21 @@ class ResNetStages:
                 ops.conv_gemm(t2, blk.w3, y, scale=blk.s3, bias=blk.b3, residual=idn, relu=True, max_ctas=max_ctas)
                 x = y
         return x
+
+    def _dcn_conv2(self, blk, t1, t2, stride, max_ctas):
+        """deformable conv2 + bn2 + ReLU as three launches: the offset conv (fp32 offsets in every mode), the sampling of
+        t1 into tap-major columns (ops.dcn_sample), and their contraction with the packed weight (K = 9 Cin)"""
+        n, ho, wo, _ = t2.shape
+        off = self._buf("dcn_off", (n, ho, wo, DCN_OFFSET_ROWS), fp32=True)
+        ops.conv_gemm(t1, blk.wo, off, taps=(3, 3), dil=blk.dil, pad=blk.dil, stride=(stride, stride), bias=blk.bo,
+                      max_ctas=max_ctas)
+        cols = self._buf("dcn_cols", (n, ho, wo, 9 * blk.mid))
+        self.cut(lambda: ops.dcn_sample(t1, off, cols, blk.modulated, stride, blk.dil))
+        ops.conv_gemm(cols, blk.w2, t2, scale=blk.s2, bias=blk.b2, relu=True, max_ctas=max_ctas)
+
+
+def _run_now(launch):
+    launch()
 
 
 class Backbone:
@@ -321,6 +371,8 @@ class Backbone:
             ops.unmark_split16(p)
             ops.pack_split16(p)          # in place: res2 reads split-fp16
         chained = self.dtype == torch.float16
+        if self.stages.has_dcn:
+            return self._forward_segments(p, out, tail, chained)
         dual = chained and ops.DUAL_CHAIN[0] and n >= ops.DUAL_MIN_IMAGES and n % 2 == 0
         with ops.chain(self._chains, ("body", tuple(p.shape), tail is not None, dual), self.dev, enabled=chained,
                        interleave=dual) as ch:
@@ -332,6 +384,38 @@ class Backbone:
                 y = self.stages.forward(p, out=out)
                 if tail is not None:
                     tail(y, None)
+        return y
+
+    def _forward_segments(self, p, out, tail, chained):
+        """res2..res4 of a body with deformable blocks. ops.chain records conv_gemm calls only, so in fp16 mode the
+        body runs as consecutive chains cut at each sampling launch: segment k ends with a block's offset conv, the
+        sampling launch follows, segment k + 1 starts with that block's contraction. `tail` rides on the last segment.
+        The interleaved two-lane form is not used for these bodies."""
+        key = ("body", tuple(p.shape), tail is not None, "dcn")
+        seg = [0, None]
+
+        def open_segment():
+            seg[1] = ops.chain(self._chains, key + (seg[0],), self.dev, enabled=chained)
+            seg[1].__enter__()
+            seg[0] += 1
+
+        def cut(launch):
+            seg[1].__exit__(None, None, None)
+            launch()
+            open_segment()
+
+        open_segment()
+        self.stages.cut = cut
+        try:
+            y = self.stages.forward(p, out=out)
+            if tail is not None:
+                tail(y, None)
+        except BaseException:
+            seg[1].__exit__(*sys.exc_info())
+            raise
+        finally:
+            self.stages.cut = _run_now
+        seg[1].__exit__(None, None, None)
         return y
 
 
@@ -730,7 +814,7 @@ class WindowedEngine(HeadCommon):
             for stages in (self.backbone.stages, self.res5):
                 for blocks in stages.stages:
                     for blk in blocks:
-                        for name in ("w1", "w2", "w3", "wd"):
+                        for name in ("w1", "w2", "w3", "wd", "wo"):
                             if getattr(blk, name, None) is not None:
                                 setattr(blk, name, ops.presplit(getattr(blk, name)))
             self.rpn_w, self.rpn_hw = ops.presplit(self.rpn_w), ops.presplit(self.rpn_hw)

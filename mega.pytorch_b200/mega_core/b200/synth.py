@@ -92,7 +92,8 @@ def _linear(sd, p, nout, nin, gen, std=None, gain=1.0):
     sd[p + "bias"] = torch.randn(nout, generator=gen) * 0.01
 
 
-def make_state_dict(arch="mega_r101", seed=0, num_classes=31, reduce_channel=False, global_res_stage=1, advanced_stage=1):
+def make_state_dict(arch="mega_r101", seed=0, num_classes=31, reduce_channel=False, global_res_stage=1, advanced_stage=1,
+                    stage_with_dcn=(False, False, False, False), modulated_dcn=False):
     """state_dict with the reference's key names/shapes for
     arch in {"mega_r101", "mega_r50", "rdn_r101", "fgfa_r101", "dff_r101", "base_r50", "base_r101", "mega_x101", "base_x101"}
     (+ "_tiny" suffix: 1 block per stage, for fast CPU tests). x101: ResNeXt-101 32x8d (NUM_GROUPS 32, WIDTH_PER_GROUP 8:
@@ -103,7 +104,11 @@ def make_state_dict(arch="mega_r101", seed=0, num_classes=31, reduce_channel=Fal
       global_res_stage MODEL.VID.MEGA.GLOBAL.RES_STAGE: g_* holds global_res_stage + 1 attention modules
       advanced_stage   MODEL.VID.ROI_BOX_HEAD.ATTENTION.ADVANCED_STAGE of RDN: 0 drops fcs.2 and attention modules 2, 3
                        (the RDN-base configs)
-    The tensors of the defaults do not depend on these options' existence; the reduction conv is drawn last."""
+      stage_with_dcn   MODEL.RESNETS.STAGE_WITH_DCN (res2..res4; res5 stays plain): conv2 of those stages becomes a
+                       DFConv2d -- its 3x3 weight moves to conv2.conv.weight and conv2.offset.{weight,bias} are added
+      modulated_dcn    MODEL.RESNETS.WITH_MODULATED_DCN: 27 offset channels (18 offsets + 9 mask logits) instead of 18
+    The tensors of the defaults do not depend on these options' existence; the reduction conv and the offset convs
+    are drawn last."""
     gen = torch.Generator().manual_seed(seed)
     tiny = arch.endswith("_tiny")
     base = arch.replace("_tiny", "")
@@ -209,8 +214,26 @@ def make_state_dict(arch="mega_r101", seed=0, num_classes=31, reduce_channel=Fal
     if reduce_channel and method in ("mega", "rdn"):
         sd[fe + "conv.weight"] = _kaiming((256, 2048, 1, 1), gen, gain=1.0)
         sd[fe + "conv.bias"] = torch.zeros(256)
+    for li in range(1, 4):
+        if stage_with_dcn[li - 1]:
+            _dcn_stage(sd, "backbone.body.layer%d." % li, gen, modulated_dcn)
     sd.pop("rpn.anchor_generator.cell_anchors.0")
     return sd
+
+
+def _dcn_stage(sd, prefix, gen, modulated):
+    """conv2 of every block of the stage as a DFConv2d (layers/misc.py:114-189). The offset conv reads the ReLU output
+    of bn1 (entries around 0.6 in magnitude); its weights are scaled so that the offsets come out with a spread of
+    about 1.5 pixels: most samples are fractional, and near the border some fall outside the map."""
+    b = 0
+    while (prefix + "%d.conv2.weight" % b) in sd:
+        p = prefix + "%d.conv2." % b
+        w = sd.pop(p + "weight")
+        sd[p + "conv.weight"] = w
+        k = 27 if modulated else 18
+        sd[p + "offset.weight"] = _kaiming((k, w.shape[1], 3, 3), gen, gain=2.0)
+        sd[p + "offset.bias"] = torch.randn(k, generator=gen) * 0.5
+        b += 1
 
 
 def global_frame_indices(seg_len, size=10, seed=0):

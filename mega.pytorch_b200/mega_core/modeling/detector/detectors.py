@@ -63,9 +63,19 @@ def build_detection_model_from_state_dict(sd, method="mega", device="cuda", prec
     while ("backbone.body.layer3.%d.conv1.weight" % n3) in sd:
         n3 += 1
     body = {6: "R-50-C4", 23: "R-101-C4"}.get(n3)
-    w2 = sd["backbone.body.layer1.0.conv2.weight"]              # [G * width, width, 3, 3]
+    l1 = "backbone.body.layer1.0.conv2."
+    w2 = sd[l1 + "conv.weight"] if (l1 + "conv.weight") in sd else sd[l1 + "weight"]     # [G * width, width, 3, 3]
     cfg = vid_config(method, body or "R-101-C4", device, num_groups=w2.shape[0] // w2.shape[1],
                      width_per_group=w2.shape[1], stride_in_1x1=stride_in_1x1)
+    # MODEL.RESNETS.STAGE_WITH_DCN / WITH_MODULATED_DCN / DEFORMABLE_GROUPS: a deformable conv2 keeps its weight as
+    # conv2.conv.weight beside the offset conv conv2.offset.* (18 or 27 output channels per deformable group)
+    offsets = [sd.get("backbone.body.layer%d.0.conv2.offset.weight" % li) for li in (1, 2, 3)]
+    if any(o is not None for o in offsets):
+        k = next(o for o in offsets if o is not None).shape[0]
+        r = cfg.MODEL.RESNETS
+        r.STAGE_WITH_DCN = tuple(o is not None for o in offsets) + (False,)
+        r.WITH_MODULATED_DCN = k % 27 == 0
+        r.DEFORMABLE_GROUPS = k // (27 if r.WITH_MODULATED_DCN else 18)
     if precision is not None:
         cfg.MODEL.B200.PRECISION = precision
     cfg.MODEL.VID.ROI_BOX_HEAD.REDUCE_CHANNEL = (fe + "conv.weight") in sd

@@ -14,7 +14,7 @@ import torch
 from torch import nn
 
 from . import registry
-from ..layers import Conv2d, FrozenBatchNorm2d
+from ..layers import Conv2d, DFConv2d, FrozenBatchNorm2d
 from ..b200 import engine as _engine
 
 BLOCKS = {"R-50-C4": (3, 4, 6), "R-101-C4": (3, 4, 23)}
@@ -48,7 +48,7 @@ def _image_size(images):
 
 
 class Bottleneck(nn.Module):
-    def __init__(self, cin, mid, cout, stride, dilation, groups=1, stride_in_1x1=True):
+    def __init__(self, cin, mid, cout, stride, dilation, groups=1, stride_in_1x1=True, dcn=None):
         super().__init__()
         if cin != cout:
             self.downsample = nn.Sequential(Conv2d(cin, cout, 1, stride=(stride if dilation == 1 else 1), bias=False),
@@ -58,18 +58,29 @@ class Bottleneck(nn.Module):
         s1, s3 = (stride, 1) if stride_in_1x1 else (1, stride)          # resnet.py:272-275
         self.conv1 = Conv2d(cin, mid, 1, stride=s1, bias=False)
         self.bn1 = FrozenBatchNorm2d(mid)
-        self.conv2 = Conv2d(mid, mid, 3, stride=s3, padding=dilation, dilation=dilation, groups=groups, bias=False)
+        if dcn is not None:         # resnet.py:286-299: dcn = (with_modulated_dcn, deformable_groups)
+            self.conv2 = DFConv2d(mid, mid, with_modulated_dcn=dcn[0], kernel_size=3, stride=s3, groups=groups,
+                                  dilation=dilation, deformable_groups=dcn[1], bias=False)
+        else:
+            self.conv2 = Conv2d(mid, mid, 3, stride=s3, padding=dilation, dilation=dilation, groups=groups, bias=False)
         self.bn2 = FrozenBatchNorm2d(mid)
         self.conv3 = Conv2d(mid, cout, 1, bias=False)
         self.bn3 = FrozenBatchNorm2d(cout)
 
 
-def _stage(cin, mid, cout, n, stride, dilation=1, groups=1, stride_in_1x1=True):
+def _stage(cin, mid, cout, n, stride, dilation=1, groups=1, stride_in_1x1=True, dcn=None):
     blocks = []
     for i in range(n):
         blocks.append(Bottleneck(cin if i == 0 else cout, mid, cout, stride if i == 0 else 1, dilation, groups,
-                                 stride_in_1x1))
+                                 stride_in_1x1, dcn))
     return nn.Sequential(*blocks)
+
+
+def stage_dcn(cfg, stage):
+    """(with_modulated_dcn, deformable_groups) of res`stage+1` when MODEL.RESNETS.STAGE_WITH_DCN marks it, else None
+    (resnet.py:110-124)"""
+    r = cfg.MODEL.RESNETS
+    return (bool(r.WITH_MODULATED_DCN), r.DEFORMABLE_GROUPS) if r.STAGE_WITH_DCN[stage - 1] else None
 
 
 def bottleneck_width(cfg, stage):
@@ -93,9 +104,12 @@ class ResNetBody(nn.Module):
         b = BLOCKS[cfg.MODEL.BACKBONE.CONV_BODY]
         g, s1x1 = cfg.MODEL.RESNETS.NUM_GROUPS, cfg.MODEL.RESNETS.STRIDE_IN_1X1
         self.stem = Stem()
-        self.layer1 = _stage(64, bottleneck_width(cfg, 1), 256, b[0], 1, groups=g, stride_in_1x1=s1x1)
-        self.layer2 = _stage(256, bottleneck_width(cfg, 2), 512, b[1], 2, groups=g, stride_in_1x1=s1x1)
-        self.layer3 = _stage(512, bottleneck_width(cfg, 3), 1024, b[2], 2, groups=g, stride_in_1x1=s1x1)
+        self.layer1 = _stage(64, bottleneck_width(cfg, 1), 256, b[0], 1, groups=g, stride_in_1x1=s1x1,
+                             dcn=stage_dcn(cfg, 1))
+        self.layer2 = _stage(256, bottleneck_width(cfg, 2), 512, b[1], 2, groups=g, stride_in_1x1=s1x1,
+                             dcn=stage_dcn(cfg, 2))
+        self.layer3 = _stage(512, bottleneck_width(cfg, 3), 1024, b[2], 2, groups=g, stride_in_1x1=s1x1,
+                             dcn=stage_dcn(cfg, 3))
         self.out_channels = 1024
 
 
@@ -388,9 +402,19 @@ def engine_config_from(cfg):
                                "width %d; the kernels serve widths in multiples of 64 and group widths 8, 16, 32 or 64)"
                                % (g, wpg, stage + 1, width, gw))
             break
-    if any(m.RESNETS.STAGE_WITH_DCN):
-        unsupported.append("MODEL.RESNETS.STAGE_WITH_DCN = %s (the engines have no deformable backbone stages)"
-                           % (tuple(m.RESNETS.STAGE_WITH_DCN),))
+    dcn = tuple(m.RESNETS.STAGE_WITH_DCN)
+    if any(dcn):
+        if dcn[3]:
+            unsupported.append("MODEL.RESNETS.STAGE_WITH_DCN = %s (the 4th entry, res5, must be False: in the C4 models "
+                               "res5 is the box head's ResNetHead, which the reference builds without a deformable "
+                               "conv, so the entry would be ignored)" % (dcn,))
+        if g > 1:
+            unsupported.append("MODEL.RESNETS.STAGE_WITH_DCN = %s with MODEL.RESNETS.NUM_GROUPS = %d (deformable "
+                               "stages are served with dense conv2, NUM_GROUPS 1)" % (dcn, g))
+        if m.RESNETS.DEFORMABLE_GROUPS != 1:
+            unsupported.append("MODEL.RESNETS.DEFORMABLE_GROUPS = %d (deformable stages are served with one deformable "
+                               "group; the reference's modulated conv slices its 18 offsets and 9 masks for one group, "
+                               "layers/misc.py:182-184)" % m.RESNETS.DEFORMABLE_GROUPS)
     att = v.ROI_BOX_HEAD.ATTENTION
     if v.METHOD == "mega":
         if not (v.MEGA.MEMORY.ENABLE and v.MEGA.GLOBAL.ENABLE):
