@@ -373,6 +373,16 @@ int mega_deform_im2col(const float* input, const float* offset, const float* mas
 int mega_dcn_sample_nhwc(const void* input, int format, int batch, int height, int width, int channels,
                          const float* offset, int offset_ld, int modulated, int stride, int dil, void* cols,
                          void* stream);
+/* The same sampling with `deformable_groups` (MODEL.RESNETS.DEFORMABLE_GROUPS, DCN v1): group g samples its
+ * channels / deformable_groups consecutive channels [g C / dg, (g + 1) C / dg) at its own offsets, channels 18 g + 2 tap
+ * and 18 g + 2 tap + 1 of the offset rows -- the reference's (b * dg + g) * 2 * kh * kw offset planes
+ * (deform_conv_kernel_cuda.cu, deformable_im2col_gpu_kernel). offset_ld >= 18 * deformable_groups;
+ * channels % deformable_groups == 0, (channels / deformable_groups) % 8 == 0, 1 <= deformable_groups <= 128; modulated
+ * sampling takes deformable_groups == 1 (then this is mega_dcn_sample_nhwc, bit for bit). Output layout, formats,
+ * alignment, stream and graph capture as above. */
+int mega_dcn_sample_nhwc_groups(const void* input, int format, int batch, int height, int width, int channels,
+                                int deformable_groups, const float* offset, int offset_ld, int modulated, int stride,
+                                int dil, void* cols, void* stream);
 
 /* ------------------- deformable position-sensitive ROI pooling forward (csrc/deform_pool.h:11-37) */
 int mega_deform_psroi_pooling_forward(const float* input, const float* rois, const float* trans, int num_rois,

@@ -1,15 +1,18 @@
 // Deformable-convolution sampling over NHWC activations into the column operand of a 1x1 GEMM: the middle launch of a
 // deformable bottleneck conv2 (MODEL.RESNETS.STAGE_WITH_DCN). The offset conv before it and the contraction after it
 // (K = 9 C, tap-major) are conv_gemm launches. One output row per pixel:
-//     cols[pixel][tap * C + c] = mask(pixel, tap) * bilinear(input, position(pixel, tap))[c]
+//     cols[pixel][tap * C + c] = mask(pixel, tap) * bilinear(input, position(pixel, tap, g))[c],   g = c / (C / dg)
 // with position = (h * stride - dil + i * dil + dh, w * stride - dil + j * dil + dw) for tap = 3 i + j (the DFConv2d
-// padding: dil), (dh, dw) = offset[pixel][2 tap], offset[pixel][2 tap + 1], and mask = sigmoid(offset[pixel][18 + tap])
-// for DCN v2, 1 for v1. The geometry and the interpolation are dcn_sample.cuh, shared with deform.cu's tile kernel.
+// padding: dil), (dh, dw) = offset[pixel][18 g + 2 tap], offset[pixel][18 g + 2 tap + 1] -- deformable group g of dg
+// samples its C / dg consecutive channels at its own 9 positions -- and mask = sigmoid(offset[pixel][18 + tap]) for
+// DCN v2 (one group), 1 for v1. The geometry and the interpolation are dcn_sample.cuh, shared with deform.cu's tile
+// kernel.
 //
-// A CTA owns kSampPix consecutive pixels: the 9 taps of each get their geometry (floor, weights, corner indices) once,
-// into shared memory; then every thread takes (pixel, tap, 8-channel chunk) items, chunk fastest. The four corners of a
-// sample are contiguous C-vectors in NHWC, so a warp reads whole corner rows with 128-bit loads and writes the
-// column row contiguously. Values are interpolated in fp32 in every storage format.
+// A CTA owns kSampPix / dg consecutive pixels (at least one): the 9 dg (tap, group) samples of each get their geometry
+// (floor, weights, corner indices) once, into dynamic shared memory -- at most 16 x 9 samples for dg <= 16, 9 dg above;
+// then every thread takes (pixel, tap, 8-channel chunk) items, chunk fastest, and reads the geometry of the chunk's
+// group. The four corners of a sample are contiguous C-vectors in NHWC, so a warp reads whole corner rows with 128-bit
+// loads and writes the column row contiguously. Values are interpolated in fp32 in every storage format.
 #include "common.cuh"
 #include "dcn_sample.cuh"
 #include "mega_b200.h"
@@ -18,6 +21,7 @@ namespace mega {
 
 constexpr int kSampPix = 16;
 constexpr int kSampThreads = 256;
+constexpr int kSampMaxGroups = 128;     // 9 x 128 samples of one pixel: 41.5 KB of geometry, under the 48 KB default
 
 struct Vec8 {
   float v[8];
@@ -78,31 +82,35 @@ __device__ __forceinline__ void store8(void* base, long long e, const float (&x)
 
 template <int FMT>
 __global__ void __launch_bounds__(kSampThreads)
-dcn_sample_nhwc_kernel(const void* __restrict__ input, int height, int width, int channels,
-                       const float* __restrict__ offset, int offset_ld, int modulated, int stride, int dil, int ho,
-                       int wo, long long pixels, void* __restrict__ cols) {
-  __shared__ DcnTap geo[kSampPix * 9];
-  __shared__ float mval[kSampPix * 9];
-  const long long p0 = static_cast<long long>(blockIdx.x) * kSampPix;
-  const int npix = static_cast<int>(min(static_cast<long long>(kSampPix), pixels - p0));
-  for (int t = threadIdx.x; t < npix * 9; t += kSampThreads) {
-    const long long pix = p0 + t / 9;
-    const int tap = t % 9, i = tap / 3, j = tap - 3 * i;
+dcn_sample_nhwc_kernel(const void* __restrict__ input, int height, int width, int channels, int groups,
+                       int cta_pix, const float* __restrict__ offset, int offset_ld, int modulated, int stride,
+                       int dil, int ho, int wo, long long pixels, void* __restrict__ cols) {
+  extern __shared__ float4 smem[];
+  DcnTap* geo = reinterpret_cast<DcnTap*>(smem);                       // [cta_pix][9][groups]
+  float* mval = reinterpret_cast<float*>(geo + cta_pix * 9 * groups);   // likewise
+  const long long p0 = static_cast<long long>(blockIdx.x) * cta_pix;
+  const int npix = static_cast<int>(min(static_cast<long long>(cta_pix), pixels - p0));
+  const int per_pix = 9 * groups;
+  for (int t = threadIdx.x; t < npix * per_pix; t += kSampThreads) {
+    const int lp = t / per_pix, r = t - lp * per_pix, tap = r / groups, grp = r - tap * groups;
+    const long long pix = p0 + lp;
+    const int i = tap / 3, j = tap - 3 * i;
     const int w_col = static_cast<int>(pix % wo), h_col = static_cast<int>((pix / wo) % ho);
     const float* o = offset + pix * offset_ld;
-    const float h_im = h_col * stride - dil + i * dil + __ldg(o + 2 * tap);
-    const float w_im = w_col * stride - dil + j * dil + __ldg(o + 2 * tap + 1);
+    const float h_im = h_col * stride - dil + i * dil + __ldg(o + 18 * grp + 2 * tap);
+    const float w_im = w_col * stride - dil + j * dil + __ldg(o + 18 * grp + 2 * tap + 1);
     geo[t] = dcn_tap_geometry(h_im, w_im, height, width);
     mval[t] = modulated ? dcn_sigmoid(__ldg(o + 18 + tap)) : 1.f;
   }
   __syncthreads();
-  const int chunks = channels >> 3;
+  const int chunks = channels >> 3, group_chunks = chunks / groups;
   const long long plane = static_cast<long long>(height) * width;
   for (int it = threadIdx.x; it < npix * 9 * chunks; it += kSampThreads) {
     const int t = it / chunks, q = it - t * chunks;
     const long long pix = p0 + t / 9;
     const int tap = t % 9;
-    const DcnTap g = geo[t];
+    const int s = t * groups + q / group_chunks;
+    const DcnTap g = geo[s];
     const long long img = pix / (static_cast<long long>(ho) * wo) * plane;      // first pixel of the image
     const int c = q * 8;
     float x[8];
@@ -121,7 +129,7 @@ dcn_sample_nhwc_kernel(const void* __restrict__ input, int height, int width, in
           for (int k = 0; k < 8; ++k) v[r].v[k] = 0.f;
         }
       }
-      const float m = mval[t];
+      const float m = mval[s];
 #pragma unroll
       for (int k = 0; k < 8; ++k) x[k] = dcn_blend(g, v[0].v[k], v[1].v[k], v[2].v[k], v[3].v[k]) * m;
     }
@@ -133,33 +141,46 @@ dcn_sample_nhwc_kernel(const void* __restrict__ input, int height, int width, in
 
 using namespace mega;
 
-extern "C" int mega_dcn_sample_nhwc(const void* input, int format, int batch, int height, int width, int channels,
-                                    const float* offset, int offset_ld, int modulated, int stride, int dil,
-                                    void* cols, void* stream_v) {
+extern "C" int mega_dcn_sample_nhwc_groups(const void* input, int format, int batch, int height, int width,
+                                           int channels, int deformable_groups, const float* offset, int offset_ld,
+                                           int modulated, int stride, int dil, void* cols, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  const int dg = deformable_groups;
   MEGA_ARG_CHECK(format == MEGA_DCN_FP32 || format == MEGA_DCN_FP16 || format == MEGA_DCN_SPLIT16,
                  "dcn_sample_nhwc: format must be MEGA_DCN_FP32, _FP16 or _SPLIT16");
   MEGA_ARG_CHECK(batch >= 0 && height > 0 && width > 0 && channels > 0 && channels % 32 == 0,
                  "dcn_sample_nhwc: channels must be a positive multiple of 32");
+  MEGA_ARG_CHECK(dg >= 1 && dg <= kSampMaxGroups && channels % dg == 0 && (channels / dg) % 8 == 0,
+                 "dcn_sample_nhwc: deformable_groups must be 1..128 and divide channels into multiples of 8");
+  MEGA_ARG_CHECK(!modulated || dg == 1, "dcn_sample_nhwc: modulated sampling takes one deformable group");
   MEGA_ARG_CHECK(stride >= 1 && dil >= 1, "dcn_sample_nhwc: stride and dilation must be >= 1");
-  MEGA_ARG_CHECK(offset_ld >= (modulated ? 27 : 18), "dcn_sample_nhwc: offset_ld smaller than the offset channels");
+  MEGA_ARG_CHECK(offset_ld >= (modulated ? 27 : 18 * dg), "dcn_sample_nhwc: offset_ld smaller than the offset channels");
   MEGA_ARG_CHECK((reinterpret_cast<uintptr_t>(input) & 15) == 0 && (reinterpret_cast<uintptr_t>(cols) & 15) == 0,
                  "dcn_sample_nhwc: input and cols must be 16-byte aligned");
   const int ho = (height - 1) / stride + 1, wo = (width - 1) / stride + 1;     // 3x3, padding = dilation
   const long long pixels = static_cast<long long>(batch) * ho * wo;
   if (pixels == 0) return MEGA_OK;
-  const long long blocks = (pixels + kSampPix - 1) / kSampPix;
+  const int cta_pix = max(1, kSampPix / dg);
+  const size_t smem = (sizeof(DcnTap) + sizeof(float)) * 9 * dg * cta_pix;
+  const long long blocks = (pixels + cta_pix - 1) / cta_pix;
   MEGA_ARG_CHECK(blocks < (1LL << 31), "dcn_sample_nhwc: grid too large");
   const unsigned grid = static_cast<unsigned>(blocks);
   if (format == MEGA_DCN_FP32)
-    dcn_sample_nhwc_kernel<MEGA_DCN_FP32><<<grid, kSampThreads, 0, stream>>>(
-        input, height, width, channels, offset, offset_ld, modulated, stride, dil, ho, wo, pixels, cols);
+    dcn_sample_nhwc_kernel<MEGA_DCN_FP32><<<grid, kSampThreads, smem, stream>>>(
+        input, height, width, channels, dg, cta_pix, offset, offset_ld, modulated, stride, dil, ho, wo, pixels, cols);
   else if (format == MEGA_DCN_FP16)
-    dcn_sample_nhwc_kernel<MEGA_DCN_FP16><<<grid, kSampThreads, 0, stream>>>(
-        input, height, width, channels, offset, offset_ld, modulated, stride, dil, ho, wo, pixels, cols);
+    dcn_sample_nhwc_kernel<MEGA_DCN_FP16><<<grid, kSampThreads, smem, stream>>>(
+        input, height, width, channels, dg, cta_pix, offset, offset_ld, modulated, stride, dil, ho, wo, pixels, cols);
   else
-    dcn_sample_nhwc_kernel<MEGA_DCN_SPLIT16><<<grid, kSampThreads, 0, stream>>>(
-        input, height, width, channels, offset, offset_ld, modulated, stride, dil, ho, wo, pixels, cols);
+    dcn_sample_nhwc_kernel<MEGA_DCN_SPLIT16><<<grid, kSampThreads, smem, stream>>>(
+        input, height, width, channels, dg, cta_pix, offset, offset_ld, modulated, stride, dil, ho, wo, pixels, cols);
   MEGA_CUDA_CHECK(cudaGetLastError());
   return MEGA_OK;
+}
+
+extern "C" int mega_dcn_sample_nhwc(const void* input, int format, int batch, int height, int width, int channels,
+                                    const float* offset, int offset_ld, int modulated, int stride, int dil,
+                                    void* cols, void* stream_v) {
+  return mega_dcn_sample_nhwc_groups(input, format, batch, height, width, channels, 1, offset, offset_ld, modulated,
+                                     stride, dil, cols, stream_v);
 }

@@ -249,6 +249,8 @@ lib.mega_vid_eval.argtypes = [_vp, _vp, _vp, _vp, _vp, _ll, _vp, _vp, _vp, _vp, 
 lib.mega_vid_eval.restype = _i
 lib.mega_dcn_sample_nhwc.argtypes = [_vp, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _vp]
 lib.mega_dcn_sample_nhwc.restype = _i
+lib.mega_dcn_sample_nhwc_groups.argtypes = [_vp, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _i, _vp, _vp]
+lib.mega_dcn_sample_nhwc_groups.restype = _i
 
 
 class JpegInfo(ctypes.Structure):
@@ -295,5 +297,6 @@ EXPORTS = [
     "mega_image_transform_u8_ex", "mega_bbox_aug_workspace_bytes", "mega_bbox_aug_collect", "mega_bbox_aug_merge",
     "mega_proposal_recall_workspace_bytes", "mega_proposal_recall",
     "mega_vid_eval_workspace_bytes", "mega_vid_eval", "mega_dcn_sample_nhwc",
+    "mega_dcn_sample_nhwc_groups",
     "mega_jpeg_probe", "mega_jpeg_entropy_decode", "mega_jpeg_plan_batch", "mega_jpeg_decode_batch",
 ]

@@ -129,7 +129,8 @@ def pack_conv(w, dev, dtype=torch.float32):
     return w.float().permute(2, 3, 0, 1).reshape(kh * kw, co, ci).contiguous().to(dev).to(dtype)
 
 
-# output rows of a deformable conv2's offset conv: its 18 (DCN v1) or 27 (v2) channels zero-padded to the narrowest N tile
+# output rows of a deformable conv2's offset conv: its 18 (DCN v1) or 27 (v2) channels zero-padded to the narrowest N tile;
+# 18 per group with several deformable groups, padded to a multiple of it (64 at 2 groups, 96 at 4, 160 at 8)
 DCN_OFFSET_ROWS = 32
 
 
@@ -192,18 +193,23 @@ class ResNetStages:
 
     @staticmethod
     def _init_dcn(blk, sd, p, w, dev, dtype):
-        """DFConv2d (layers/misc.py:114-189) with one deformable group: conv2.offset, a 3x3 conv with bias whose 18 (v1)
-        or 27 (v2, modulated) output channels are zero-padded to DCN_OFFSET_ROWS; conv2.conv, the deformable conv, packed
-        [1, Cout, 9 Cin] tap-major for the contraction over the sampled columns (K = 9 Cin)"""
+        """DFConv2d (layers/misc.py:114-189): conv2.offset, a 3x3 conv with bias whose output channels -- 18 per
+        deformable group (v1) or 27 (v2, modulated, one group) -- are zero-padded to a multiple of DCN_OFFSET_ROWS;
+        conv2.conv, the deformable conv, packed [1, Cout, 9 Cin] tap-major for the contraction over the sampled columns
+        (K = 9 Cin)"""
         wo, bo = sd[p + "conv2.offset.weight"].float(), sd[p + "conv2.offset.bias"].float()
         k, ci = wo.shape[0], wo.shape[1]
-        assert blk.groups == 1 and k in (18, 27) and tuple(wo.shape[2:]) == (3, 3), \
-            "%sconv2: deformable conv2 is served dense, with one deformable group (offset channels %d)" % (p, k)
         blk.modulated = k == 27
-        wpad = torch.zeros(DCN_OFFSET_ROWS, ci, 3, 3)
+        blk.dg = 1 if blk.modulated else k // 18
+        assert (blk.groups == 1 and tuple(wo.shape[2:]) == (3, 3) and (blk.modulated or k % 18 == 0)
+                and ci % blk.dg == 0 and ci // blk.dg % 8 == 0), \
+            ("%sconv2: deformable conv2 is served dense, v2 with one deformable group, v1 with deformable groups of a "
+             "multiple of 8 channels (offset channels %d, %d input channels)" % (p, k, ci))
+        rows = blk.off_rows = -(-k // DCN_OFFSET_ROWS) * DCN_OFFSET_ROWS
+        wpad = torch.zeros(rows, ci, 3, 3)
         wpad[:k] = wo
         blk.wo = pack_conv(wpad, dev, dtype)
-        bpad = torch.zeros(DCN_OFFSET_ROWS)
+        bpad = torch.zeros(rows)
         bpad[:k] = bo
         blk.bo = bpad.to(dev)
         co = w.shape[0]
@@ -300,11 +306,13 @@ class ResNetStages:
         """deformable conv2 + bn2 + ReLU as three launches: the offset conv (fp32 offsets in every mode), the sampling of
         t1 into tap-major columns (ops.dcn_sample), and their contraction with the packed weight (K = 9 Cin)"""
         n, ho, wo, _ = t2.shape
-        off = self._buf("dcn_off", (n, ho, wo, DCN_OFFSET_ROWS), fp32=True)
+        off = self._buf("dcn_off", (n, ho, wo, blk.off_rows), fp32=True)
         ops.conv_gemm(t1, blk.wo, off, taps=(3, 3), dil=blk.dil, pad=blk.dil, stride=(stride, stride), bias=blk.bo,
                       max_ctas=max_ctas)
         cols = self._buf("dcn_cols", (n, ho, wo, 9 * blk.mid))
-        self.cut(lambda: ops.dcn_sample(t1, off, cols, blk.modulated, stride, blk.dil))
+        # one deformable group goes in as the plain call (stand-ins for ops.dcn_sample without the keyword serve it)
+        kw = {"deformable_groups": blk.dg} if blk.dg > 1 else {}
+        self.cut(lambda: ops.dcn_sample(t1, off, cols, blk.modulated, stride, blk.dil, **kw))
         ops.conv_gemm(cols, blk.w2, t2, scale=blk.s2, bias=blk.b2, relu=True, max_ctas=max_ctas)
 
 

@@ -825,11 +825,12 @@ def maxpool3x3s2(x, out):
     return out
 
 
-def dcn_sample(x, offset, cols, modulated, stride=1, dil=1):
+def dcn_sample(x, offset, cols, modulated, stride=1, dil=1, deformable_groups=1):
     """deformable 3x3 sampling (padding = dil) of x [N,H,W,C] NHWC (fp32, fp16 or split-fp16) at the positions of
-    offset [N,Ho,Wo,>=18 / 27] fp32 (conv_gemm's output of the offset conv) into cols [N,Ho,Wo,9*C] in x's format,
-    tap-major (include/mega_b200.h, mega_dcn_sample_nhwc). Not a conv_gemm: it runs between chain segments, never
-    inside an open chain."""
+    offset [N,Ho,Wo,>=18 dg / 27] fp32 (conv_gemm's output of the offset conv) into cols [N,Ho,Wo,9*C] in x's format,
+    tap-major (include/mega_b200.h, mega_dcn_sample_nhwc_groups). deformable_groups = dg (DCN v1): channel group g of
+    C / dg samples at offset channels 18 g ... 18 g + 17. Not a conv_gemm: it runs between chain segments, never inside
+    an open chain."""
     require_cuda(x, offset, cols)
     assert _CHAIN_MODE[0] is None, "dcn_sample inside an open ops.chain would run before the chain's layers"
     n, h, w, c = x.shape
@@ -838,8 +839,9 @@ def dcn_sample(x, offset, cols, modulated, stride=1, dil=1):
     assert tuple(cols.shape) == (n, (h - 1) // stride + 1, (w - 1) // stride + 1, 9 * c)
     assert tuple(offset.shape[:3]) == tuple(cols.shape[:3])
     fmt = 1 if x.dtype == torch.float16 else (2 if is_split16(x) else 0)
-    check(lib.mega_dcn_sample_nhwc(ptr(x), fmt, n, h, w, c, ptr(offset), offset.shape[3], 1 if modulated else 0,
-                                   stride, dil, ptr(cols), stream_ptr()), "mega_dcn_sample_nhwc")
+    check(lib.mega_dcn_sample_nhwc_groups(ptr(x), fmt, n, h, w, c, deformable_groups, ptr(offset), offset.shape[3],
+                                          1 if modulated else 0, stride, dil, ptr(cols), stream_ptr()),
+          "mega_dcn_sample_nhwc_groups")
     LAUNCHES[0] += 1
     return cols
 

@@ -93,7 +93,7 @@ def _linear(sd, p, nout, nin, gen, std=None, gain=1.0):
 
 
 def make_state_dict(arch="mega_r101", seed=0, num_classes=31, reduce_channel=False, global_res_stage=1, advanced_stage=1,
-                    stage_with_dcn=(False, False, False, False), modulated_dcn=False):
+                    stage_with_dcn=(False, False, False, False), modulated_dcn=False, deformable_groups=1):
     """state_dict with the reference's key names/shapes for
     arch in {"mega_r101", "mega_r50", "rdn_r101", "fgfa_r101", "dff_r101", "base_r50", "base_r101", "mega_x101", "base_x101"}
     (+ "_tiny" suffix: 1 block per stage, for fast CPU tests). x101: ResNeXt-101 32x8d (NUM_GROUPS 32, WIDTH_PER_GROUP 8:
@@ -107,8 +107,10 @@ def make_state_dict(arch="mega_r101", seed=0, num_classes=31, reduce_channel=Fal
       stage_with_dcn   MODEL.RESNETS.STAGE_WITH_DCN (res2..res4; res5 stays plain): conv2 of those stages becomes a
                        DFConv2d -- its 3x3 weight moves to conv2.conv.weight and conv2.offset.{weight,bias} are added
       modulated_dcn    MODEL.RESNETS.WITH_MODULATED_DCN: 27 offset channels (18 offsets + 9 mask logits) instead of 18
+      deformable_groups MODEL.RESNETS.DEFORMABLE_GROUPS (DCN v1 only): 18 offset channels per group, group g in rows
+                       18 g .. 18 g + 17; group 0 is the one-group offset conv, groups 1.. are drawn after it
     The tensors of the defaults do not depend on these options' existence; the reduction conv and the offset convs
-    are drawn last."""
+    are drawn last, the offset convs of groups 1.. after every other tensor."""
     gen = torch.Generator().manual_seed(seed)
     tiny = arch.endswith("_tiny")
     base = arch.replace("_tiny", "")
@@ -214,9 +216,13 @@ def make_state_dict(arch="mega_r101", seed=0, num_classes=31, reduce_channel=Fal
     if reduce_channel and method in ("mega", "rdn"):
         sd[fe + "conv.weight"] = _kaiming((256, 2048, 1, 1), gen, gain=1.0)
         sd[fe + "conv.bias"] = torch.zeros(256)
+    assert deformable_groups == 1 or not modulated_dcn, "several deformable groups are a DCN v1 setting"
+    dcn_convs = []
     for li in range(1, 4):
         if stage_with_dcn[li - 1]:
-            _dcn_stage(sd, "backbone.body.layer%d." % li, gen, modulated_dcn)
+            dcn_convs += _dcn_stage(sd, "backbone.body.layer%d." % li, gen, modulated_dcn)
+    for p in dcn_convs:
+        _dcn_groups(sd, p, gen, deformable_groups)
     sd.pop("rpn.anchor_generator.cell_anchors.0")
     return sd
 
@@ -224,8 +230,10 @@ def make_state_dict(arch="mega_r101", seed=0, num_classes=31, reduce_channel=Fal
 def _dcn_stage(sd, prefix, gen, modulated):
     """conv2 of every block of the stage as a DFConv2d (layers/misc.py:114-189). The offset conv reads the ReLU output
     of bn1 (entries around 0.6 in magnitude); its weights are scaled so that the offsets come out with a spread of
-    about 1.5 pixels: most samples are fractional, and near the border some fall outside the map."""
+    about 1.5 pixels: most samples are fractional, and near the border some fall outside the map. Returns the conv2
+    prefixes."""
     b = 0
+    convs = []
     while (prefix + "%d.conv2.weight" % b) in sd:
         p = prefix + "%d.conv2." % b
         w = sd.pop(p + "weight")
@@ -233,7 +241,18 @@ def _dcn_stage(sd, prefix, gen, modulated):
         k = 27 if modulated else 18
         sd[p + "offset.weight"] = _kaiming((k, w.shape[1], 3, 3), gen, gain=2.0)
         sd[p + "offset.bias"] = torch.randn(k, generator=gen) * 0.5
+        convs.append(p)
         b += 1
+    return convs
+
+
+def _dcn_groups(sd, p, gen, groups):
+    """offset conv rows of deformable groups 1 .. groups - 1 of the DFConv2d at p, each drawn as group 0 was"""
+    w, bias = [sd[p + "offset.weight"]], [sd[p + "offset.bias"]]
+    for _ in range(1, groups):
+        w.append(_kaiming(tuple(w[0].shape), gen, gain=2.0))
+        bias.append(torch.randn(bias[0].shape[0], generator=gen) * 0.5)
+    sd[p + "offset.weight"], sd[p + "offset.bias"] = torch.cat(w), torch.cat(bias)
 
 
 def global_frame_indices(seg_len, size=10, seed=0):

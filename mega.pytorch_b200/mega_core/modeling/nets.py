@@ -411,10 +411,16 @@ def engine_config_from(cfg):
         if g > 1:
             unsupported.append("MODEL.RESNETS.STAGE_WITH_DCN = %s with MODEL.RESNETS.NUM_GROUPS = %d (deformable "
                                "stages are served with dense conv2, NUM_GROUPS 1)" % (dcn, g))
-        if m.RESNETS.DEFORMABLE_GROUPS != 1:
-            unsupported.append("MODEL.RESNETS.DEFORMABLE_GROUPS = %d (deformable stages are served with one deformable "
-                               "group; the reference's modulated conv slices its 18 offsets and 9 masks for one group, "
-                               "layers/misc.py:182-184)" % m.RESNETS.DEFORMABLE_GROUPS)
+        dg = m.RESNETS.DEFORMABLE_GROUPS
+        widths = [bottleneck_width(cfg, stage) for stage in (1, 2, 3) if dcn[stage - 1]]
+        if dg != 1 and m.RESNETS.WITH_MODULATED_DCN:
+            unsupported.append("MODEL.RESNETS.DEFORMABLE_GROUPS = %d with MODEL.RESNETS.WITH_MODULATED_DCN (modulated "
+                               "stages are served with one deformable group; the reference's modulated conv slices its "
+                               "18 offsets and 9 masks for one group, layers/misc.py:182-184)" % dg)
+        elif dg < 1 or any(c % dg or c // dg % 8 for c in widths):
+            unsupported.append("MODEL.RESNETS.DEFORMABLE_GROUPS = %d (each deformable group samples a multiple of 8 "
+                               "channels: the group count must divide every deformable stage's conv2 width, here %s, "
+                               "into multiples of 8)" % (dg, "/".join(str(c) for c in widths)))
     att = v.ROI_BOX_HEAD.ATTENTION
     if v.METHOD == "mega":
         if not (v.MEGA.MEMORY.ENABLE and v.MEGA.GLOBAL.ENABLE):
