@@ -587,6 +587,8 @@ static int roi_align_nhwc_launch(const T* input, int channels, int height, int w
                                  long long out_roi_stride, cudaStream_t stream) {
   constexpr int V = Vec16<T>::N;
   constexpr int kSlice = kRoiSliceBytes / static_cast<int>(sizeof(T));
+  MEGA_ARG_CHECK(pooled_h > 0 && pooled_w > 0 && channels > 0 && height > 0 && width > 0,
+                 "roi_align_nhwc: bad pooled size / channels / map size");
   MEGA_ARG_CHECK((channels % V) == 0, "roi_align_nhwc: channels must be a multiple of 16 bytes");
   MEGA_ARG_CHECK((reinterpret_cast<uintptr_t>(input) & 15) == 0 && (reinterpret_cast<uintptr_t>(output) & 15) == 0 &&
                      (out_roi_stride % V) == 0 && (in_img_stride % V) == 0,
@@ -623,7 +625,8 @@ extern "C" int mega_roi_align_forward_nchw(const float* input, int batch, int ch
                                            int pooled_w, int sampling_ratio, float* output, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   (void)batch;
-  MEGA_ARG_CHECK(pooled_h > 0 && pooled_w > 0 && channels > 0, "roi_align: bad pooled size / channels");
+  MEGA_ARG_CHECK(pooled_h > 0 && pooled_w > 0 && channels > 0 && height > 0 && width > 0,
+                 "roi_align: bad pooled size / channels / map size");
   const long long total = static_cast<long long>(num_rois) * channels * pooled_h * pooled_w;
   if (total == 0) return MEGA_OK;  // ROIAlign_cuda.cu:278-281
   long long blocks = (total + 255) / 256;
@@ -651,6 +654,8 @@ extern "C" int mega_roi_align_forward_nhwc_f16(const void* input, int channels, 
                                                int pooled_w, int sampling_ratio, void* output,
                                                long long out_roi_stride, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  MEGA_ARG_CHECK(pooled_h > 0 && pooled_w > 0 && channels > 0 && height > 0 && width > 0,
+                 "roi_align_nhwc_f16: bad pooled size / channels / map size");
   // fast path: 128-channel slices, up to 7x7 bins
   const bool fast = (channels % 128) == 0 && pooled_h <= 7 && pooled_w <= 7 &&
                     (reinterpret_cast<uintptr_t>(input) & 15) == 0 && (reinterpret_cast<uintptr_t>(output) & 15) == 0 &&
@@ -695,7 +700,7 @@ extern "C" int mega_roi_align_forward_nhwc_split16(const void* input, int channe
                                                    long long out_roi_stride, void* stream_v) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   MEGA_ARG_CHECK((channels % 128) == 0 && pooled_h <= 7 && pooled_w <= 7 && pooled_h > 0 && pooled_w > 0 &&
-                     height <= kSepMaxDim && width <= kSepMaxDim,
+                     height <= kSepMaxDim && width <= kSepMaxDim && height > 0 && width > 0,
                  "roi_align_split16: needs channels %% 128 == 0, bins <= 7x7, map <= 64x64 (got C %d, %dx%d bins, map %dx%d)",
                  channels, pooled_h, pooled_w, height, width);
   MEGA_ARG_CHECK((reinterpret_cast<uintptr_t>(input) & 127) == 0 && (reinterpret_cast<uintptr_t>(output) & 127) == 0 &&

@@ -773,6 +773,19 @@ def roi_align_nhwc(feat, boxes, roi_batch, scale, ph, pw, sampling_ratio, out):
     n, h, w, c = feat.shape
     k = boxes.shape[0]
     assert out.dtype == feat.dtype
+    # the kernels address a pixel as image * stride(0) + (y * W + x) * C, a box as row * stride(0) + column, and a pooled
+    # value as roi * stride(0) + bin * C + channel: any other layout would be read or written silently wrong
+    if any(s != d for s, d, m in zip(feat.stride()[1:], (w * c, c, 1), (h, w, c)) if m > 1):
+        raise _lib.MegaError("roi_align_nhwc: feat must be dense NHWC within an image (strides %s)" % (feat.stride(),))
+    if boxes.dtype != torch.float32 or boxes.dim() != 2 or boxes.shape[1] < 4 or (k and boxes.stride(1) != 1):
+        raise _lib.MegaError("roi_align_nhwc: boxes must be fp32 [K, 4] with unit column stride (%s, %s, strides %s)" % (
+            boxes.dtype, tuple(boxes.shape), boxes.stride()))
+    if roi_batch is not None and (roi_batch.dtype != torch.int32 or not roi_batch.is_contiguous() or roi_batch.numel() < k):
+        raise _lib.MegaError("roi_align_nhwc: roi_batch must be contiguous int32 with >= %d entries (%s, %d)" % (
+            k, roi_batch.dtype, roi_batch.numel()))
+    if out.dim() != 2 or (k and out.stride(1) != 1) or out.shape[0] < k or out.shape[1] < ph * pw * c:
+        raise _lib.MegaError("roi_align_nhwc: out must hold %d rows of %d values with unit inner stride (%s, strides %s)" % (
+            k, ph * pw * c, tuple(out.shape), out.stride()))
     fn = lib.mega_roi_align_forward_nhwc_f16 if feat.dtype == torch.float16 else lib.mega_roi_align_forward_nhwc
     if is_split16(feat):
         # split-fp16 map -> split-fp16 rows (marks `out`); maps beyond the separable kernel's 64 x 64 cells go through fp32
@@ -780,6 +793,9 @@ def roi_align_nhwc(feat, boxes, roi_batch, scale, ph, pw, sampling_ratio, out):
             fn = lib.mega_roi_align_forward_nhwc_split16
             mark_split16(out)
         else:
+            if not out.is_contiguous():       # packed in place below
+                raise _lib.MegaError("roi_align_nhwc: a split-fp16 map above 64 x 64 cells, or bins above 7 x 7, needs a "
+                                     "contiguous out")
             plain = unpack_split16(feat.contiguous(), torch.empty_like(feat))
             unmark_split16(out)
             roi_align_nhwc(plain, boxes, roi_batch, scale, ph, pw, sampling_ratio, out)
