@@ -244,6 +244,9 @@ extern "C" int mega_box_postprocess(const float* logits, int ld_logits, const fl
   MEGA_ARG_CHECK(r_max >= 1 && r_max <= kMaxRois, "box_postprocess: r_max must be in [1, %d]", kMaxRois);
   MEGA_ARG_CHECK(num_classes >= 2, "box_postprocess: need at least one foreground class");
   MEGA_ARG_CHECK(count_ptr != nullptr, "box_postprocess: count_ptr is null");
+  MEGA_ARG_CHECK(reinterpret_cast<uintptr_t>(proposals) % 16 == 0, "box_postprocess: proposals must be 16-byte aligned");
+  MEGA_ARG_CHECK(ld_logits >= num_classes && ld_deltas >= 4 * num_classes, "box_postprocess: row pitches %d / %d below "
+                 "%d logits / %d deltas", ld_logits, ld_deltas, num_classes, 4 * num_classes);
   const long long need = mega_box_postprocess_workspace_bytes(r_max, num_classes);
   MEGA_ARG_CHECK(workspace && workspace_bytes >= need, "box_postprocess: workspace too small (%lld < %lld)",
                  workspace_bytes, need);

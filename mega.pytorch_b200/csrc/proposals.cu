@@ -605,7 +605,7 @@ extern "C" int mega_nms(const float* boxes, const float* scores, int n, float th
 }
 
 extern "C" long long mega_rpn_select_workspace_bytes(int n_img, int h, int w, int num_anchors, int pre_nms) {
-  if (pre_nms > kNmsMaxBoxes || n_img < 1) return -1;
+  if (pre_nms > kNmsMaxBoxes || n_img < 1 || h < 0 || w < 0 || num_anchors < 1) return -1;
   const size_t n = static_cast<size_t>(h) * w * num_anchors;
   const size_t k = pre_nms < static_cast<int>(n) ? pre_nms : n;
   const size_t cb = (k + 63) / 64;
@@ -630,7 +630,11 @@ extern "C" int mega_rpn_select(const float* head, long long head_img_stride, int
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   MEGA_ARG_CHECK(pre_nms > 0 && pre_nms <= kNmsMaxBoxes, "rpn_select: pre_nms_top_n must be in (0, %d]", kNmsMaxBoxes);
   MEGA_ARG_CHECK(post_nms > 0, "rpn_select: post_nms_top_n must be positive");
+  MEGA_ARG_CHECK(n_img >= 1, "rpn_select: n_img=%d, need at least one image", n_img);
+  MEGA_ARG_CHECK(h >= 0 && w >= 0 && num_anchors >= 1, "rpn_select: %d x %d cells x %d anchors", h, w, num_anchors);
   MEGA_ARG_CHECK(ld >= 5 * num_anchors, "rpn_select: head row must hold A logits + 4A deltas");
+  MEGA_ARG_CHECK(out_boxes != nullptr && out_scores != nullptr && out_count != nullptr, "rpn_select: null output");
+  MEGA_ARG_CHECK(reinterpret_cast<uintptr_t>(out_boxes) % 16 == 0, "rpn_select: out_boxes must be 16-byte aligned");
   const long long need = mega_rpn_select_workspace_bytes(n_img, h, w, num_anchors, pre_nms);
   MEGA_ARG_CHECK(workspace != nullptr && workspace_bytes >= need, "rpn_select: workspace too small (%lld < %lld)",
                  workspace_bytes, need);
@@ -685,11 +689,15 @@ extern "C" int mega_rpn_select(const float* head, long long head_img_stride, int
                                                                reinterpret_cast<float4*>(out_boxes), out_scores,
                                                                out_anchor, out_count);
   } else {
-    dim3 grid(cb, cb, n_img);
-    nms_mask_kernel<<<grid, 64, 0, stream>>>(p.sorted_boxes, kNmsMaxBoxes, nullptr, k, nms_thresh, mask,
-                                             static_cast<long long>(k) * cb, cb);
-    nms_sweep_kernel<<<n_img, 128, 0, stream>>>(mask, static_cast<long long>(k) * cb, p.valid, kNmsMaxBoxes, nullptr, k,
-                                                cb, post_nms, kept_pos, kNmsMaxBoxes, kept_count);
+    if (k > 0) {
+      dim3 grid(cb, cb, n_img);
+      nms_mask_kernel<<<grid, 64, 0, stream>>>(p.sorted_boxes, kNmsMaxBoxes, nullptr, k, nms_thresh, mask,
+                                               static_cast<long long>(k) * cb, cb);
+      nms_sweep_kernel<<<n_img, 128, 0, stream>>>(mask, static_cast<long long>(k) * cb, p.valid, kNmsMaxBoxes, nullptr,
+                                                  k, cb, post_nms, kept_pos, kNmsMaxBoxes, kept_count);
+    } else {   // an empty map: nothing kept, rpn_write_kernel zero-fills the outputs as the greedy kernel does
+      MEGA_CUDA_CHECK(cudaMemsetAsync(kept_count, 0, sizeof(int) * n_img, stream));
+    }
     rpn_write_kernel<<<n_img, 256, 0, stream>>>(p.sorted_boxes, p.sorted_scores, p.sorted_anchor, kept_pos, kNmsMaxBoxes,
                                                 kept_count, post_nms, reinterpret_cast<float4*>(out_boxes), out_scores,
                                                 out_anchor, out_count);

@@ -710,14 +710,21 @@ def _workspace(key, nbytes, device):
 
 def nms_device(boxes, scores, thresh, keep=None, count=None):
     """-> (keep int64 [n] buffer, count int32 [1]) on the device; no synchronisation."""
-    require_cuda(boxes, scores)
+    require_cuda(boxes, scores, keep, count)
     n = boxes.shape[0]
+    if boxes.dim() != 2 or boxes.shape[1] != 4 or scores.numel() != n:
+        raise _lib.MegaError("nms: boxes must be [n, 4] with n scores (%s, %d scores)" % (tuple(boxes.shape), scores.numel()))
     boxes = boxes.contiguous().float()
     scores = scores.contiguous().float()
     if keep is None:
         keep = torch.empty(max(n, 1), dtype=torch.int64, device=boxes.device)
     if count is None:
         count = torch.zeros(1, dtype=torch.int32, device=boxes.device)
+    # the kernels write up to n int64 indices into keep and one int32 into count, both densely
+    if keep.dtype != torch.int64 or not keep.is_contiguous() or keep.numel() < n:
+        raise _lib.MegaError("nms: keep must be contiguous int64 with >= %d entries (%s, %d)" % (n, keep.dtype, keep.numel()))
+    if count.dtype != torch.int32 or count.numel() < 1:
+        raise _lib.MegaError("nms: count must be int32 with >= 1 entry (%s)" % (count.dtype,))
     nbytes = lib.mega_nms_workspace_bytes(n)
     if nbytes < 0:
         raise _lib.MegaError("nms: n=%d exceeds the single-pass capacity (8192 boxes)" % n)
@@ -735,6 +742,15 @@ def rpn_select(head, n_img, h, w, base_anchors, im_w, im_h, pre_nms, post_nms, n
     a = base_anchors.shape[0]
     ld = head.shape[-1]
     dev = head.device
+    # the kernels read logit a of cell (y, x) of image i at i * stride(0) + (y * w + x) * ld + a, and anchor shape a at a * 4
+    if (head.dtype != torch.float32 or head.dim() != 4 or head.shape[0] < n_img or tuple(head.shape[1:3]) != (h, w)
+            or any(st != d for st, d, m in zip(head.stride()[1:], (w * ld, ld, 1), (h, w, ld)) if m > 1)):
+        raise _lib.MegaError("rpn_select: head must be fp32 [>= %d, %d, %d, ld], dense within an image (%s, %s, strides %s)"
+                             % (n_img, h, w, head.dtype, tuple(head.shape), head.stride()))
+    if base_anchors.dtype != torch.float32 or base_anchors.dim() != 2 or base_anchors.shape[1] != 4 \
+            or not base_anchors.is_contiguous():
+        raise _lib.MegaError("rpn_select: base_anchors must be contiguous fp32 [A, 4] (%s, %s)" % (
+            base_anchors.dtype, tuple(base_anchors.shape)))
     if out is None:
         boxes = torch.empty(n_img, post_nms, 4, device=dev)
         scores = torch.empty(n_img, post_nms, device=dev)
@@ -742,9 +758,20 @@ def rpn_select(head, n_img, h, w, base_anchors, im_w, im_h, pre_nms, post_nms, n
         anchor = torch.empty(n_img, post_nms, dtype=torch.int32, device=dev) if want_anchor else None
     else:
         boxes, scores, anchor, count = out
+        require_cuda(boxes, scores, anchor, count)
+    # the outputs are written densely, row i * post + j; the boxes as float4
+    for name, t, dtype, shape in (("boxes", boxes, torch.float32, (n_img, post_nms, 4)),
+                                  ("scores", scores, torch.float32, (n_img, post_nms)),
+                                  ("anchor", anchor, torch.int32, (n_img, post_nms)), ("count", count, torch.int32, (n_img,))):
+        if t is not None and (t.dtype != dtype or tuple(t.shape) != shape or not t.is_contiguous()):
+            raise _lib.MegaError("rpn_select: %s must be contiguous %s %s (%s, %s)" % (name, dtype, shape, t.dtype,
+                                                                                   tuple(t.shape)))
+    if boxes.data_ptr() % 16:
+        raise _lib.MegaError("rpn_select: boxes must be 16-byte aligned (stored as float4)")
     nbytes = lib.mega_rpn_select_workspace_bytes(n_img, h, w, a, pre_nms)
     if nbytes < 0:
-        raise _lib.MegaError("rpn_select: pre_nms_top_n=%d exceeds 8192" % pre_nms)
+        raise _lib.MegaError("rpn_select: %d images of %d x %d cells x %d anchors, pre_nms_top_n=%d: out of range "
+                             "(n_img >= 1, h, w >= 0, A >= 1, pre_nms_top_n <= 8192)" % (n_img, h, w, a, pre_nms))
     ws = _workspace("rpn%d" % n_img, nbytes, dev)
     check(lib.mega_rpn_select(ptr(head), head.stride(0), ld, n_img, h, w, a, stride, ptr(base_anchors), float(im_w),
                               float(im_h), pre_nms, post_nms, float(nms_thresh), float(min_size), ptr(ws), ws.numel(),
@@ -979,8 +1006,27 @@ def box_postprocess(logits, deltas, proposals, count, num_classes, im_w, im_h, s
     nbytes = lib.mega_box_postprocess_workspace_bytes(r, num_classes)
     if nbytes < 0:
         raise _lib.MegaError("box_postprocess: at most 512 proposals per image")
-    ws = _workspace("post", nbytes, logits.device)
     ob, os_, ol, oc = out
+    require_cuda(ob, os_, ol, oc)
+    # the kernels read proposal r as a float4 at r * 4, logit c of row r at r * stride(0) + c (deltas likewise), and
+    # write detection i at i * 4 / i of the three outputs
+    if proposals.dtype != torch.float32 or proposals.dim() != 2 or proposals.shape[1] != 4 or not proposals.is_contiguous() \
+            or proposals.data_ptr() % 16:
+        raise _lib.MegaError("box_postprocess: proposals must be contiguous 16-byte aligned fp32 [R, 4] (%s, %s)" % (
+            proposals.dtype, tuple(proposals.shape)))
+    for name, t, cols in (("logits", logits, num_classes), ("deltas", deltas, 4 * num_classes)):
+        if t.dtype != torch.float32 or t.dim() != 2 or t.shape[0] < r or t.shape[1] < cols or (cols > 1 and t.stride(1) != 1):
+            raise _lib.MegaError("box_postprocess: %s must be fp32 [>= %d, >= %d] with unit inner stride (%s, %s, strides %s)"
+                                 % (name, r, cols, t.dtype, tuple(t.shape), t.stride()))
+    if count.dtype != torch.int32 or count.numel() < 1:
+        raise _lib.MegaError("box_postprocess: count must be an int32 device scalar (%s)" % (count.dtype,))
+    cap = ob.shape[0]
+    for name, t, dtype, shape in (("boxes", ob, torch.float32, (cap, 4)), ("scores", os_, torch.float32, (cap,)),
+                                  ("labels", ol, torch.int64, (cap,)), ("count", oc, torch.int32, (1,))):
+        if t.dtype != dtype or tuple(t.shape) != shape or not t.is_contiguous():
+            raise _lib.MegaError("box_postprocess: out %s must be contiguous %s %s (%s, %s)" % (
+                name, dtype, shape, t.dtype, tuple(t.shape)))
+    ws = _workspace("post", nbytes, logits.device)
     check(lib.mega_box_postprocess(ptr(logits), logits.stride(0), ptr(deltas), deltas.stride(0), ptr(proposals),
                                    ptr(count), r, num_classes, float(im_w), float(im_h), float(score_thresh),
                                    float(nms_thresh), max_det, *[float(x) for x in weights], ptr(ws), ws.numel(),

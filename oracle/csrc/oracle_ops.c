@@ -18,10 +18,14 @@
 
 typedef struct { float score; int64_t idx; } scored_t;
 
-/* descending by score; ties by ascending index (stable) */
+/* descending by score; ties by ascending index (stable). A NaN score ranks above every number and NaNs tie with
+ * each other, as in torch.sort(descending=True) and the device's key order (a positive NaN has the largest key). */
 static int cmp_scored(const void* a, const void* b) {
   const scored_t* x = (const scored_t*)a;
   const scored_t* y = (const scored_t*)b;
+  const int xn = isnan(x->score), yn = isnan(y->score);
+  if (xn != yn) return xn ? -1 : 1;
+  if (xn) return (x->idx > y->idx) - (x->idx < y->idx);
   if (x->score > y->score) return -1;
   if (x->score < y->score) return 1;
   return (x->idx > y->idx) - (x->idx < y->idx);
