@@ -286,7 +286,8 @@ int mega_relation_softmax_f16(float* logits, void* probs_f16, int n_rows, int ld
 
 /* the position-biased soft-max with Wg [16,64], bg [16] and dim_mat [8] given as HOST arrays: they travel in the
  * kernel parameters, so every weight is a constant-bank operand (no shared-memory traffic); probs_f16 may be NULL
- * (probabilities in place, fp32). Same arithmetic as mega_relation_softmax. */
+ * (probabilities in place, fp32). Same arithmetic as mega_relation_softmax. ldm <= 7168: a row of more than 1024 keys
+ * keeps its logits in the shared memory of a 2-CTA cluster (longer rows: the device-weight entry points). */
 int mega_relation_softmax_pe(float* logits, void* probs_f16, int n_rows, int ldm, const float* boxes_q,
                              const float* boxes_k, const float* wg_host, const float* bg_host,
                              const float* dim_mat_host, const int* m_valid_ptr, int m_host, const int* n_valid_ptr,

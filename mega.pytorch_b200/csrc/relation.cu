@@ -7,9 +7,10 @@
 // Here nothing of that is materialised: for every (query n, key m) pair the four log-ratios,
 // the 64 sin/cos features, the 64->16 projection, ReLU, log and the scaled logit are computed in
 // registers and the soft-max is taken in place over the [G,N,M] logits produced by the
-// wgmma Q.K^T GEMM. One CTA per query row; two passes over its [16,M] slice (L2-resident):
-// logits + online (max, sum), then normalise.
+// wgmma Q.K^T GEMM. One CTA per query row (a 2-CTA cluster for rows of more than 1024 keys with the weights in the
+// kernel parameters); two passes over its [16,M] slice: logits + online (max, sum), then normalise.
 #include <stdlib.h>
+#include <cooperative_groups.h>
 #include <cuda_fp16.h>
 #include "common.cuh"
 #include "mega_b200.h"
@@ -228,11 +229,11 @@ struct RelParamsW {
   float inv_dim[8];
 };
 
-template <bool SMEM_STAGE>
+template <bool SMEM_STAGE>   // SMEM_STAGE = false: the 2-CTA specialisation below
 __global__ void __launch_bounds__(kRelThreads)
 relation_softmax_pe_kernel(const __grid_constant__ RelParamsW pw) {
   const RelParams& p = pw.b;
-  extern __shared__ float stage_s[];   // [16][ldm] when SMEM_STAGE
+  extern __shared__ float stage_s[];   // [16][ldm]
   __shared__ float red_max[kRelThreads / 32][kGroups];
   __shared__ float red_sum[kRelThreads / 32][kGroups];
   __shared__ float fin_max[kGroups], fin_inv[kGroups];
@@ -297,7 +298,7 @@ relation_softmax_pe_kernel(const __grid_constant__ RelParamsW pw) {
     for (int g = 0; g < kGroups; ++g) {
       const float b = __logf(__fadd_rn(fmaxf(bias[g], 0.f), 1e-6f));
       const float l = __fadd_rn(b, __fmul_rn(p.scale, lg[g]));
-      if (SMEM_STAGE) stage_s[g * p.ldm + m] = l; else srow[g * p.head_stride + m] = l;
+      stage_s[g * p.ldm + m] = l;
       // online (max, sum) with one exp: e = exp(-|l - mx|)
       const float d = l - mx[g];
       const float e = __expf(-fabsf(d));
@@ -340,7 +341,7 @@ relation_softmax_pe_kernel(const __grid_constant__ RelParamsW pw) {
     if (p.p16 && p.p_split) {
 #pragma unroll
       for (int g = 0; g < kGroups; ++g) {
-        const float l = SMEM_STAGE ? stage_s[g * p.ldm + (m < m_valid ? m : 0)] : srow[g * p.head_stride + m];
+        const float l = stage_s[g * p.ldm + (m < m_valid ? m : 0)];
         const float pr = (m < m_valid) ? __expf(l - fin_max[g]) * fin_inv[g] : 0.f;
         store_prob16<true>(p.p16, static_cast<long long>(n) * p.ldm + g * p.head_stride + m, pr);
       }
@@ -348,7 +349,7 @@ relation_softmax_pe_kernel(const __grid_constant__ RelParamsW pw) {
 #pragma unroll
       for (int g = 0; g < kGroups; ++g) {
         float* sp = srow + g * p.head_stride + m;
-        const float l = SMEM_STAGE ? stage_s[g * p.ldm + (m < m_valid ? m : 0)] : *sp;
+        const float l = stage_s[g * p.ldm + (m < m_valid ? m : 0)];
         const float pr = (m < m_valid) ? __expf(l - fin_max[g]) * fin_inv[g] : 0.f;
         if (p.p16) p.p16[static_cast<long long>(n) * p.ldm + g * p.head_stride + m] = __float2half_rn(pr);
         else *sp = pr;
@@ -563,6 +564,175 @@ relation_softmax_mma_kernel(const __grid_constant__ RelParamsW pw) {
   }
 }
 
+// ---- relation_softmax_pe_kernel<false>: rows of more than 1024 keys with the weights in the kernel parameters. A
+// query row's [16, ldm] fp32 logits (241 KB at MEGA stage 0's 3776 keys) do not fit in one CTA's shared memory, so the
+// row runs as a 2-CTA cluster and CTA r keeps heads 8r .. 8r+7 ([8, ldm], 121 KB) in its own shared memory (the
+// "shared-memory stage" is split across the cluster). The position bias of a (query, key) pair
+// is one product for all 16 heads, so each CTA computes it for half of the keys and writes the other CTA's 8 heads
+// into that CTA's shared memory (DSMEM): no sin / cos is evaluated twice, the global logits are read once and the
+// probabilities written once (relation_softmax_kernel<false> writes the biased logits back to global memory and reads
+// them again: three times the logits' bytes more through HBM).
+// The per-pair arithmetic is the primary template's, and the (max, sum) statistics are accumulated from shared memory
+// in its order -- thread t of 256 takes keys t, t + 256, ... and the
+// partials are reduced over the same lanes and then the same 8 warps; the four 256-thread quarters of the CTA run
+// that order on 2 heads each. 1024 threads (64 registers): the shared memory allows one CTA per SM, and the
+// position-bias loop, which bounds the kernel, needs the warps to hide its latencies (measured on H100 SXM at MEGA
+// stage 0's 675 x 3776: 0.36 ms with 1024 threads, 0.40 ms with 512, 0.39 ms as 4-CTA clusters of 256 threads).
+constexpr int kPairCtas = 2;
+constexpr int kPairThreads = 1024;
+constexpr int kPairHeads = kGroups / kPairCtas;                            // heads per CTA
+constexpr int kPairMaxLdm = 224 * 1024 / (kPairHeads * static_cast<int>(sizeof(float)));   // 224 of a CTA's 227 KB
+
+template <>
+__global__ void __cluster_dims__(kPairCtas, 1, 1) __launch_bounds__(kPairThreads)
+relation_softmax_pe_kernel<false>(const __grid_constant__ RelParamsW pw) {
+  namespace cg = cooperative_groups;
+  const RelParams& p = pw.b;
+  extern __shared__ float stage_s[];   // [kPairHeads][ldm]: heads kPairHeads * rank .. of the row
+  __shared__ float red_max[kRelThreads / 32][kPairHeads];
+  __shared__ float red_sum[kRelThreads / 32][kPairHeads];
+  __shared__ float fin_max[kPairHeads], fin_inv[kPairHeads];
+
+  cg::cluster_group cluster = cg::this_cluster();
+  const int rank = static_cast<int>(cluster.block_rank());
+  const int n = blockIdx.x / kPairCtas;
+  const int tid = threadIdx.x;
+  const int ldm = p.ldm;
+  const int m_valid = p.m_valid_ptr ? min(*p.m_valid_ptr, ldm) : p.m_host;
+  if (p.n_valid_ptr) {
+    const int nv = *p.n_valid_ptr;
+    if (n >= nv && n < p.n_valid_off) return;   // both CTAs of the cluster see the same row: both leave
+  }
+  float* head_s[kPairCtas];   // shared memory of the CTA that owns heads kPairHeads * r ..
+#pragma unroll
+  for (int r = 0; r < kPairCtas; ++r) head_s[r] = cluster.map_shared_rank(stage_s, r);
+  const float4 q = *reinterpret_cast<const float4*>(p.boxes_q + static_cast<long long>(n) * 4);
+  const float qw = __fadd_rn(__fsub_rn(q.z, q.x), 1.f);
+  const float qh = __fadd_rn(__fsub_rn(q.w, q.y), 1.f);
+  const float qcx = __fmul_rn(0.5f, __fadd_rn(q.x, q.z));
+  const float qcy = __fmul_rn(0.5f, __fadd_rn(q.y, q.w));
+  float* srow = p.s + static_cast<long long>(n) * ldm;
+  cluster.sync();   // the peer has started: its shared memory may be written
+
+  // ---- biased logits of this CTA's keys (32-key blocks alternating between the CTAs), all 16 heads
+  for (int i = tid;; i += kPairThreads) {
+    const int m = (i >> 5) * (32 * kPairCtas) + rank * 32 + (i & 31);
+    if (m >= m_valid) break;
+    float lg[kGroups];
+#pragma unroll
+    for (int g = 0; g < kGroups; ++g) lg[g] = srow[g * p.head_stride + m];
+    const float4 k = *reinterpret_cast<const float4*>(p.boxes_k + static_cast<long long>(m) * 4);
+    const float kw = __fadd_rn(__fsub_rn(k.z, k.x), 1.f);
+    const float kh = __fadd_rn(__fsub_rn(k.w, k.y), 1.f);
+    const float kcx = __fmul_rn(0.5f, __fadd_rn(k.x, k.z));
+    const float kcy = __fmul_rn(0.5f, __fadd_rn(k.y, k.w));
+    float delta[4];
+    delta[0] = logf(__fadd_rn(fabsf(__fdiv_rn(__fsub_rn(qcx, kcx), qw)), 1e-3f));
+    delta[1] = logf(__fadd_rn(fabsf(__fdiv_rn(__fsub_rn(qcy, kcy), qh)), 1e-3f));
+    delta[2] = logf(__fdiv_rn(qw, kw));
+    delta[3] = logf(__fdiv_rn(qh, kh));
+    float bias[kGroups];
+#pragma unroll
+    for (int g = 0; g < kGroups; ++g) bias[g] = pw.bg[g];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const float d100 = __fmul_rn(delta[c], 100.0f);
+#pragma unroll
+      for (int kf = 0; kf < 8; ++kf) {
+        const float q0 = __fmul_rn(d100, pw.inv_dim[kf]);
+        const float rem = __fmaf_rn(-q0, pw.dim[kf], d100);
+        const float arg = __fmaf_rn(rem, pw.inv_dim[kf], q0);
+        const float kq = rintf(arg * 0.15915494309189535f);
+        float r = fmaf(-kq, 6.28125f, arg);
+        r = fmaf(-kq, 1.9353071795864769e-3f, r);
+        const float sv = __sinf(r), cv = __cosf(r);
+#pragma unroll
+        for (int g = 0; g < kGroups; ++g) {
+          bias[g] = fmaf(pw.wg[(c * 16 + kf) * kGroups + g], sv, fmaf(pw.wg[(c * 16 + 8 + kf) * kGroups + g], cv, bias[g]));
+        }
+      }
+    }
+#pragma unroll
+    for (int g = 0; g < kGroups; ++g) {
+      const float b = __logf(__fadd_rn(fmaxf(bias[g], 0.f), 1e-6f));
+      const float l = __fadd_rn(b, __fmul_rn(p.scale, lg[g]));
+      head_s[g / kPairHeads][(g % kPairHeads) * ldm + m] = l;
+    }
+  }
+  cluster.sync();   // every key of both halves is in place; no DSMEM access after this point
+
+  // ---- online (max, sum) of local heads kHp * part .. kHp * part + kHp - 1 in the primary template's order
+  constexpr int kHp = kPairHeads / (kPairThreads / kRelThreads);
+  const int t = tid & (kRelThreads - 1), part = tid / kRelThreads;
+  const int lane = t & 31, warp = t >> 5;
+  float mx[kHp], sm[kHp];
+#pragma unroll
+  for (int j = 0; j < kHp; ++j) {
+    mx[j] = -INFINITY;
+    sm[j] = 0.f;
+  }
+  for (int m = t; m < m_valid; m += kRelThreads) {
+#pragma unroll
+    for (int j = 0; j < kHp; ++j) {
+      const float l = stage_s[(part * kHp + j) * ldm + m];
+      const float d = l - mx[j];
+      const float e = __expf(-fabsf(d));
+      sm[j] = (d > 0.f) ? fmaf(sm[j], e, 1.f) : (sm[j] + e);
+      mx[j] = fmaxf(mx[j], l);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < kHp; ++j) {
+    float m_ = mx[j], s_ = sm[j];
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const float om = __shfl_xor_sync(0xffffffffu, m_, off);
+      const float os = __shfl_xor_sync(0xffffffffu, s_, off);
+      const float nm = fmaxf(m_, om);
+      const float a = (m_ == -INFINITY) ? 0.f : s_ * __expf(m_ - nm);
+      const float b = (om == -INFINITY) ? 0.f : os * __expf(om - nm);
+      s_ = a + b;
+      m_ = nm;
+    }
+    if (lane == 0) {
+      red_max[warp][part * kHp + j] = m_;
+      red_sum[warp][part * kHp + j] = s_;
+    }
+  }
+  __syncthreads();
+  if (tid < kPairHeads) {
+    float m_ = -INFINITY;
+    for (int w = 0; w < kRelThreads / 32; ++w) m_ = fmaxf(m_, red_max[w][tid]);
+    float s_ = 0.f;
+    for (int w = 0; w < kRelThreads / 32; ++w)
+      if (red_max[w][tid] != -INFINITY) s_ += red_sum[w][tid] * __expf(red_max[w][tid] - m_);
+    fin_max[tid] = m_;
+    fin_inv[tid] = 1.0f / s_;
+  }
+  __syncthreads();
+
+  // ---- normalise this CTA's heads; padded key columns get probability 0
+  const long long row0 = static_cast<long long>(n) * ldm + rank * kPairHeads * p.head_stride;
+  for (int m = tid; m < ldm; m += kPairThreads) {
+    if (p.p16 && p.p_split) {
+#pragma unroll
+      for (int h = 0; h < kPairHeads; ++h) {
+        const float l = stage_s[h * ldm + (m < m_valid ? m : 0)];
+        const float pr = (m < m_valid) ? __expf(l - fin_max[h]) * fin_inv[h] : 0.f;
+        store_prob16<true>(p.p16, row0 + h * p.head_stride + m, pr);
+      }
+    } else {
+#pragma unroll
+      for (int h = 0; h < kPairHeads; ++h) {
+        const float l = stage_s[h * ldm + (m < m_valid ? m : 0)];
+        const float pr = (m < m_valid) ? __expf(l - fin_max[h]) * fin_inv[h] : 0.f;
+        if (p.p16) p.p16[row0 + h * p.head_stride + m] = __float2half_rn(pr);
+        else p.s[row0 + h * p.head_stride + m] = pr;
+      }
+    }
+  }
+}
+
 // No position term: one warp per (head, query row); the row (<= 1024 keys) stays in registers, so the
 // logits are read once and the probabilities written once.
 __global__ void __launch_bounds__(256)
@@ -704,6 +874,8 @@ static int relation_softmax_pe_impl(float* logits, void* probs_f16, int p_split,
   MEGA_ARG_CHECK(logits != nullptr && n_rows >= 0 && ldm > 0 && boxes_q && boxes_k && wg_host && bg_host && dim_mat_host,
                  "relation_softmax_pe: bad arguments");
   MEGA_ARG_CHECK(m_valid_ptr != nullptr || (m_host >= 0 && m_host <= ldm), "relation_softmax_pe: m out of range");
+  MEGA_ARG_CHECK(ldm <= kPairMaxLdm, "relation_softmax_pe: ldm %d over %d keys (the device-weight entry points take it)",
+                 ldm, kPairMaxLdm);
   if (n_rows == 0) return MEGA_OK;
   RelParamsW pw;
   RelParams& p = pw.b;
@@ -741,17 +913,18 @@ static int relation_softmax_pe_impl(float* logits, void* probs_f16, int p_split,
                                          kGroups * 1024 * static_cast<int>(sizeof(float))));
     MEGA_CUDA_CHECK(cudaFuncSetAttribute(relation_softmax_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          kGroups * 1024 * static_cast<int>(sizeof(float))));
+    MEGA_CUDA_CHECK(cudaFuncSetAttribute(relation_softmax_pe_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kPairHeads * kPairMaxLdm * static_cast<int>(sizeof(float))));
     configured = true;
   }
-  const int smem = kGroups * ldm * static_cast<int>(sizeof(float));
   // measured (B200, 675 query rows): keys <= 1024 (logits staged in smem) 60 us with the tensor-core bias vs 70 us
-  // with FFMAs; 3750 keys (two passes over 163 MB of fp32 logits in global memory: bandwidth-bound) 250 vs 242 us
+  // with FFMAs. Above 1024 keys the 2-CTA kernel (H100, MEGA stage 0, 675 x 3776: see DESIGN.md section 4).
   if (use_mma && ldm <= 1024) {
-    relation_softmax_mma_kernel<true><<<n_rows, kRelThreads, smem, stream>>>(pw);
+    relation_softmax_mma_kernel<true><<<n_rows, kRelThreads, kGroups * ldm * sizeof(float), stream>>>(pw);
   } else if (ldm <= 1024) {
-    relation_softmax_pe_kernel<true><<<n_rows, kRelThreads, smem, stream>>>(pw);
+    relation_softmax_pe_kernel<true><<<n_rows, kRelThreads, kGroups * ldm * sizeof(float), stream>>>(pw);
   } else {
-    relation_softmax_pe_kernel<false><<<n_rows, kRelThreads, 0, stream>>>(pw);
+    relation_softmax_pe_kernel<false><<<kPairCtas * n_rows, kPairThreads, kPairHeads * ldm * sizeof(float), stream>>>(pw);
   }
   MEGA_CUDA_CHECK(cudaGetLastError());
   return MEGA_OK;

@@ -964,6 +964,9 @@ def transpose_2d(x, out, n_img, rows, cols):
     return out
 
 
+RELATION_PE_MAX_KEYS = 7168     # csrc/relation.cu kPairMaxLdm
+
+
 def relation_softmax(logits, n_rows, ldm, scale, boxes_q=None, boxes_k=None, wg=None, bg=None, dim_mat=None,
                      m_valid=None, m_host=0, n_valid=None, n_valid_off=0, probs_f16=None, host_w=None):
     """in place over fp32 logits [16, n_rows, ldm]; with probs_f16 (fp16, same shape) the probabilities go there -- or, when
@@ -971,7 +974,9 @@ def relation_softmax(logits, n_rows, ldm, scale, boxes_q=None, boxes_k=None, wg=
     split = probs_f16 is not None and probs_f16.dtype == torch.float32
     if split:
         assert is_split16(probs_f16) and probs_f16.numel() == logits.numel() and ldm % 32 == 0
-    if host_w is not None and boxes_q is not None:
+    # above RELATION_PE_MAX_KEYS a row's logits do not fit in the shared memory of the host-weight kernels' 2-CTA
+    # cluster: such rows take the device-weight entry points (two passes over the logits in global memory)
+    if host_w is not None and boxes_q is not None and (ldm <= RELATION_PE_MAX_KEYS or wg is None):
         # (wg [16,64], bg [16], dim_mat [8]) as contiguous fp32 HOST tensors: they travel in the kernel parameters
         require_cuda(logits, boxes_q, boxes_k, m_valid, n_valid, probs_f16)
         wg_h, bg_h, dim_h = host_w
