@@ -73,6 +73,9 @@ class EngineConfig:
     # MODEL.RESNETS.STRIDE_IN_1X1: which conv of res3 / res4's first bottleneck carries the stride, the 1x1 conv1 (True,
     # the MSRA layout) or the 3x3 conv2 (False, the layout of the Caffe2 / fb.torch ResNe(X)t and torchvision weights)
     stride_in_1x1 = True
+    # MEGA: MODEL.VID.MEGA.MEMORY.ENABLE. False (the paper's ablation without long-range memory) relates every stage's
+    # queries to the local window only: no memory rings, no pushes, key counts of 1875 / 375 instead of 3750 / 750
+    memory = True
 
     def __init__(self, **kw):
         for k, v in kw.items():
@@ -968,7 +971,8 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
     (detector/generalized_rcnn_mega.py:137-225; extractors :657-699, :754-774, :806-829, :885-933).
     Served layouts: ATTENTION.STAGE = 3 local stages; MEGA.GLOBAL.RES_STAGE = 1 (configs/MEGA/vid_R_101_C4_MEGA_1x.yaml:
     a second global stage G1 after the local ones) or 0 (vid_R_50_C4_MEGA_1x.yaml: the key rows of stage 2 go to the
-    predictor); with or without REDUCE_CHANNEL."""
+    predictor); with or without REDUCE_CHANNEL; with or without the long-range memory (MEGA.MEMORY.ENABLE, cfg.memory:
+    without it the stages relate their queries to the 1875 / 375 local rows and nothing is pushed)."""
     MAX_FRAMES_PER_STEP = 8      # key frames whose per-frame branch stepn_batched may run as one batch
 
     def __init__(self, sd, cfg=None, device="cuda"):
@@ -977,7 +981,8 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
         super().__init__(sd, cfg, dev)
         c = cfg
         self.R, self.A, self.L, self.KP = c.ref_post_nms_top_n, c.advanced_num, c.all_frame_interval, c.post_nms_top_n
-        self.GF, self.MEMF = c.global_size, c.memory_size
+        self.GF = c.global_size
+        self.MEMF = c.memory_size if c.memory else 0              # memory ring capacity in frames
         assert c.stage == 3 and c.global_res_stage in (0, 1), "engine is laid out for STAGE=3, GLOBAL.RES_STAGE 0 or 1"
         R, A, L, KP, GF = self.R, self.A, self.L, self.KP, self.GF
         res = c.pooler_resolution
@@ -1206,10 +1211,11 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
             tn[off["slot_new"][0]] = slot_new
         if gslot is not None:
             put("dst_glob", gslot * R + ar["R"])
-        mslot = self.mem_pushed % self.MEMF
-        put("dst_mem0", KP + self.nl0 + mslot * R + ar["R"])
-        put("dst_mem12", self.nq + mslot * A + ar["A"])
-        put("dst_memb12", self.nl12 + mslot * A + ar["A"])
+        if self.MEMF:
+            mslot = self.mem_pushed % self.MEMF
+            put("dst_mem0", KP + self.nl0 + mslot * R + ar["R"])
+            put("dst_mem12", self.nq + mslot * A + ar["A"])
+            put("dst_memb12", self.nl12 + mslot * A + ar["A"])
         tn[off["slot_key"][0]] = kslot
         self.tab_d.copy_(self.tab_h, non_blocking=True)
         ev = torch.cuda.Event()
@@ -1366,6 +1372,8 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
         KP, R, A, L, D = self.KP, self.R, self.A, self.L, self.feat_dim
         if not new_local:
             self._fill_tables()
+        if mode == "state" and not self.MEMF:
+            return None         # without memory a foreign key frame leaves nothing behind but its ring slots
         nl0, nl12, nq = self.nl0, self.nl12, self.nq
         kcnt, mv = self._assemble_window()
         if mode != "fused":
@@ -1422,14 +1430,20 @@ class MegaEngine(WindowedEngine, WavefrontMixin):
         return self.cur_cnt.view(-1)[:1], t("mvalid")
 
     def _push_mem0(self):
-        """update_memory(0): the oldest local frame's 75 globally enhanced rows (extractors :678-688)"""
+        """update_memory(0): the oldest local frame's 75 globally enhanced rows (extractors :678-688); nothing without
+        memory (extractors :913-917)"""
+        if not self.MEMF:
+            return
         KP, R, t = self.KP, self.R, self._tab
         with ops.copy_batch():
             ops.copy_rows(self.E0[KP:KP + R], self.E0, R, dst_idx=t("dst_mem0"))
             ops.copy_rows(self.B0[KP:KP + R], self.B0, R, dst_idx=t("dst_mem0"))
 
     def _push_mem12(self, Y, B):
-        """update_memory(1 / 2): the first 15 distilled rows of the stage that was just read (extractors :924-928)"""
+        """update_memory(1 / 2): the first 15 distilled rows of the stage that was just read (extractors :924-928);
+        nothing without memory"""
+        if not self.MEMF:
+            return
         KP, A, t = self.KP, self.A, self._tab
         with ops.copy_batch():
             ops.copy_rows(Y[KP:KP + A], Y, A, dst_idx=t("dst_mem12"))

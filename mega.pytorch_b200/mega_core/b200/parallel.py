@@ -58,16 +58,19 @@ def wave_tables(mem_pushed, rank, world, rows0, rows12, mem_frames, base0, base1
 
     mem_pushed : frames pushed into the memory before the group (identical on all ranks)
     rows0 / rows12 : rows per frame of the stage-0 memory (75) / of the stage-1 and stage-2 memories (15)
-    mem_frames : ring capacity in frames (25)
+    mem_frames : ring capacity in frames (25); 0 without a long-range memory: the schedule has no increment stages, so
+        the tables are empty and every frame sees no memory
     base0 / base12 / baseb12 : first ring row inside the stage-0 feature+box buffers, the stage-1/2 feature buffers and
         the stage-1/2 box buffers
     Returns int32 numpy arrays; entry [g * rows + j] is the destination row of row j of frame g's increment, or -1
     (= skipped by mega_copy_rows): `pre*` hold the frames g < rank, `post*` the frames g >= rank.
     `valid[g]` = memory frames frame g sees (the soft-max's key count is local rows + valid * rows)."""
     import numpy as np
-    assert 0 <= rank < world <= mem_frames, "a group must fit the memory ring (its frames take distinct slots)"
+    assert 0 <= rank < world and (mem_frames == 0 or world <= mem_frames), \
+        "a group must fit the memory ring (its frames take distinct slots)"
     out = {}
-    for name, rows, base in (("0", rows0, base0), ("12", rows12, base12), ("b12", rows12, baseb12)):
+    stages = (("0", rows0, base0), ("12", rows12, base12), ("b12", rows12, baseb12)) if mem_frames else ()
+    for name, rows, base in stages:
         pre = np.full(world * rows, -1, dtype=np.int32)
         post = np.full(world * rows, -1, dtype=np.int32)
         for g in range(world):

@@ -5,7 +5,9 @@ rows per frame) travel in one small all-gather per relation stage; before stage 
 increments of the group's earlier frames, after its last read the rest (the reference's "read, then push" order). This
 replaces the replicated "state" part of dist_step (~0.7 ms per foreign frame) by three latency-bound collectives. The
 launches of the rank's own frame are those of MegaEngine._aggregate_split(owner), so detections are bit-identical to
-dist_step for any world size. Schedule tables, the NCCL / in-process drivers and the self-check live in parallel.py; the
+dist_step for any world size. Without a long-range memory (MEGA.MEMORY.ENABLE False) the schedule has no increment
+stages: a rank aggregates its key frame from the gathered payloads alone, with the same segments and no collective
+between them. Schedule tables, the NCCL / in-process drivers and the self-check live in parallel.py; the
 evidence (symbolic proof, engine code on CPU stand-ins, gloo, bit-identity on one GPU) is listed in DESIGN.md section 6."""
 import torch
 
@@ -29,10 +31,13 @@ class WavefrontMixin:
         R, A = self.R, self.A
         z = lambda *s, dtype=torch.float32: torch.zeros(*s, device=self.dev, dtype=dtype)
         self.w_ld = self.fw + 4                              # 32-bit words per increment row: feature row | box
-        self.w_inc = [z(R, self.w_ld), z(A, self.w_ld), z(A, self.w_ld)]
-        self.w_all = [z(world, R * self.w_ld), z(world, A * self.w_ld), z(world, A * self.w_ld)]
+        # one increment per memory stage (rows per frame); none without a long-range memory
+        rows = (R, A, A) if self.MEMF else ()
+        self.w_inc = [z(n, self.w_ld) for n in rows]
+        self.w_all = [z(world, n * self.w_ld) for n in rows]
         self._wtab_off, off = {}, 0
-        for name, n in (("pre0", R), ("post0", R), ("pre12", A), ("post12", A), ("preb12", A), ("postb12", A)):
+        tables = (("pre0", R), ("post0", R), ("pre12", A), ("post12", A), ("preb12", A), ("postb12", A)) if rows else ()
+        for name, n in tables:
             self._wtab_off[name] = (off, world * n)
             off += world * n
         self._wtab_ring = [torch.zeros(off, dtype=torch.int32).pin_memory() for _ in range(4)]
@@ -47,6 +52,8 @@ class WavefrontMixin:
     def _wave_fill(self, rank, world):
         """destination-row tables of this group (host -> pinned ring -> device), from the memory counter at group start"""
         from . import parallel
+        if not self.w_inc:
+            return
         tabs = parallel.wave_tables(self.mem_pushed, rank, world, self.R, self.A, self.MEMF, self.KP + self.nl0, self.nq,
                                     self.nl12)
         ring = self._wave_steps % len(self._wtab_ring)
@@ -68,6 +75,8 @@ class WavefrontMixin:
         return x, w[:, self.fw:]
 
     def _wave_pack(self, stage, x_rows, box_rows):
+        if stage >= len(self.w_inc):
+            return
         x, b = self._inc_views(self.w_inc[stage])
         n = x.shape[0]
         with ops.copy_batch():
@@ -76,6 +85,8 @@ class WavefrontMixin:
 
     def _wave_apply(self, stage, which, x_dst, box_dst):
         """scatter the gathered increments of the group into the memory rings; `which`: "pre" / "post" """
+        if stage >= len(self.w_inc):
+            return
         x, b = self._inc_views(self.w_all[stage])
         n = x.shape[0]
         with ops.copy_batch():
@@ -150,7 +161,8 @@ class WavefrontMixin:
 
     def _wave(self, imgs, im_w, im_h, rank, world, payload=None):
         """generator of one wavefront step of rank `rank`: yields (tensor to all-gather, gathered output buffer) four
-        times -- frame payloads, then the stage-0 / 1 / 2 memory increments -- and returns the Detections of key frame
+        times -- frame payloads, then the stage-0 / 1 / 2 memory increments; once, the payloads, without a long-range
+        memory -- and returns the Detections of key frame
         `rank` of the group. `payload`: this rank's frame payload computed elsewhere (tests), instead of `imgs`.
         parallel.drive() runs it over NCCL, parallel.play() over all ranks in one process."""
         self._wave_alloc(world)
@@ -166,12 +178,10 @@ class WavefrontMixin:
         for g in range(rank + 1):                       # the window as of the own key frame
             self._wave_ingest(payloads[g])
         key = (im_w, im_h, rank, world)
-        self._wave_seg("a", key, im_w, im_h)
-        yield self.w_inc[0], self.w_all[0]
-        self._wave_seg("b", key, im_w, im_h)
-        yield self.w_inc[1], self.w_all[1]
-        self._wave_seg("c", key, im_w, im_h)
-        yield self.w_inc[2], self.w_all[2]
+        for stage, seg in enumerate("abc"):
+            self._wave_seg(seg, key, im_w, im_h)
+            if stage < len(self.w_inc):                 # a schedule without memory has no increment stages
+                yield self.w_inc[stage], self.w_all[stage]
         det = self._wave_seg("d", key, im_w, im_h)
         for g in range(rank + 1, world):                # the later frames of the group: state only
             self._wave_ingest(payloads[g])

@@ -423,9 +423,10 @@ def engine_config_from(cfg):
                                "into multiples of 8)" % (dg, "/".join(str(c) for c in widths)))
     att = v.ROI_BOX_HEAD.ATTENTION
     if v.METHOD == "mega":
-        if not (v.MEGA.MEMORY.ENABLE and v.MEGA.GLOBAL.ENABLE):
-            unsupported.append("MODEL.VID.MEGA.MEMORY.ENABLE / GLOBAL.ENABLE = False (MegaEngine is laid out for memory + "
-                               "global aggregation, generalized_rcnn_mega.py:36-40)")
+        if not v.MEGA.GLOBAL.ENABLE:
+            unsupported.append("MODEL.VID.MEGA.GLOBAL.ENABLE = False (the reference cannot run it at test time: "
+                               "MEGAFeatureExtractor._forward_test reads global_res_stage, which it sets only when the "
+                               "global stage is enabled, roi_box_feature_extractors.py:542-545)")
         if att.STAGE != 3:
             unsupported.append("MODEL.VID.ROI_BOX_HEAD.ATTENTION.STAGE = %d (MegaEngine runs 3 local stages)" % att.STAGE)
         if v.MEGA.GLOBAL.RES_STAGE not in (0, 1):
@@ -468,4 +469,5 @@ def engine_config_from(cfg):
         num_classes=m.ROI_BOX_HEAD.NUM_CLASSES,
         precision=os.environ.get("MEGA_B200_PRECISION", m.B200.PRECISION if "B200" in m else "f16"),
         **({"rpn_only": True} if m.RPN_ONLY else {}),
+        **({"memory": False} if v.METHOD == "mega" and not v.MEGA.MEMORY.ENABLE else {}),
         **({} if m.RESNETS.STRIDE_IN_1X1 else {"stride_in_1x1": False}))
