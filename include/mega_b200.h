@@ -326,7 +326,20 @@ int mega_box_postprocess(const float* logits, int ld_logits, const float* deltas
  * aggregate: resample (bilinear, border; generalized_rcnn_fgfa.py:45-62) of the cached [feats | embedding] maps of
  *   the window frames along `flow` [n_frames][h*w][flow_ld] fp32, cosine-similarity weights against the key frame's
  *   warped embedding, soft-max over frames, weighted sum of the warped feats (:64-76, :206-214) -> out [h*w][out_ld];
- *   weights_out (optional) [n_frames][h*w] fp32. */
+ *   weights_out (optional) [n_frames][h*w] fp32. n_frames <= 32, embed_channels <= 4096 (16 per thread).
+ * Layout contract (nothing here is checked by the kernels; ops.py rejects other views): every NHWC map is addressed as
+ *   base + ((n * H + y) * W + x) * ld + channel, so rows and images are packed at the map's ld and channels have unit
+ *   stride. pool_image: image and out contiguous. build_pairs: ring slots dense [hq][wq][4] at slot_stride, pairs
+ *   contiguous with n_frames entries; channels 3 and 7 of pairs are written 0. aggregate: ring slot s at
+ *   s * slot_stride, pixel stride ld >= feat_channels + embed_channels; flow frame f (window position, not slot) at
+ *   f * h * w * flow_ld; only flow channels 0 (x) and 1 (y) are read; out rows at out_ld >= feat_channels; weights_out
+ *   dense [n_frames][h][w]. avgpool2_nhwc: images at H * W * in_ld resp. ceil(H/2) * ceil(W/2) * out_ld; the divisor is
+ *   the number of cells of the 2x2 window inside the map.
+ * Warp geometry (aggregate and dff_warp_scale), fp32, one rounding per operation in this order (h, w >= 2):
+ *   gx = (fx + x) / ((w - 1) * 0.5) - 1;  px = fma(gx + 1, w, -1) * 0.5;  px = min(max(px, 0), w - 1);
+ *   x0 = floor(px), x1 = min(x0 + 1, w - 1), lx = px - x0 (the same in y); corner weights (1-lx)(1-ly), lx(1-ly),
+ *   (1-lx)ly, lx*ly. This is F.grid_sample(bilinear, padding_mode="border", align_corners=False) on the grid that
+ *   get_grid() normalises for align_corners=True, so a zero flow is not the identity. */
 int mega_fgfa_pool_image(const float* image, int height, int width, void* out, int f16, void* stream);
 int mega_fgfa_build_pairs(const void* ring, long long slot_stride, const int* slots, int n_frames, int key_pos, int hq,
                           int wq, void* pairs, int f16, void* stream);
@@ -338,7 +351,8 @@ int mega_fgfa_aggregate(const void* ring, long long slot_stride, int ld, int fea
 
 /* DFF (configs/DFF, SURVEY section 8f row 4): out[h*w][out_ld] = resample(key_feats [h*w][ld], flow [h*w][flow_ld] fp32)
  * * scale [h*w][scale_ld] -- bilinear / border warp of the key frame's feature map along the flow, times FlowNetS's
- * scale map (detector/generalized_rcnn_dff.py:41-58, :131-134). channels % 8 == 0; f16 as above. */
+ * scale map (detector/generalized_rcnn_dff.py:41-58, :131-134). channels % 8 == 0; f16 as above. Rows of key_feats,
+ * flow, scale and out are packed at their ld (pixel p at p * ld); the warp geometry is the one of the FGFA aggregate. */
 int mega_dff_warp_scale(const void* key_feats, int ld, int channels, const float* flow, int flow_ld, const void* scale,
                         long long scale_ld, int height, int width, void* out, long long out_ld, int f16, void* stream);
 

@@ -91,7 +91,10 @@ __global__ void avgpool2_nhwc_kernel(const T* __restrict__ in, int n_img, int he
 // One CTA per output pixel. ring: [slots][h*w][ld] with feats in [0, cf) and embeddings in [cf, cf + ce).
 // flow [L][h*w][flow_ld] fp32 (x, y in feature cells). Sampling = F.grid_sample(bilinear, border, align_corners=False) of
 // the grid get_grid() builds: gx = (fx + x) / ((w-1)/2) - 1  ->  pixel coordinate ((gx + 1) * w - 1) / 2, clamped to
-// [0, w-1].
+// [0, w-1]. The rounding sequence is spelled with intrinsics so that no contraction choice of the compiler changes it:
+// one fp32 rounding per operation, and (gx + 1) * w - 1 as one FMA (F.grid_sample rounds the product and the
+// difference separately; the two orders pick positions one ulp apart). The products with 0.5f are exact and stay plain
+// (an __fmul_rn there changes the instruction schedule, not the result). tests/fgfa_ref.py restates it bit for bit.
 constexpr int kAggThreads = 256;
 constexpr int kAggMaxFrames = 32;
 
@@ -101,10 +104,10 @@ struct Corner {
 };
 
 __device__ __forceinline__ Corner flow_corners(float fx, float fy, int x, int y, int w, int h, int ld) {
-  const float gx = __fdiv_rn(fx + static_cast<float>(x), static_cast<float>(w - 1) * 0.5f) - 1.0f;
-  const float gy = __fdiv_rn(fy + static_cast<float>(y), static_cast<float>(h - 1) * 0.5f) - 1.0f;
-  float px = ((gx + 1.0f) * static_cast<float>(w) - 1.0f) * 0.5f;
-  float py = ((gy + 1.0f) * static_cast<float>(h) - 1.0f) * 0.5f;
+  const float gx = __fadd_rn(__fdiv_rn(__fadd_rn(fx, static_cast<float>(x)), static_cast<float>(w - 1) * 0.5f), -1.0f);
+  const float gy = __fadd_rn(__fdiv_rn(__fadd_rn(fy, static_cast<float>(y)), static_cast<float>(h - 1) * 0.5f), -1.0f);
+  float px = __fmaf_rn(__fadd_rn(gx, 1.0f), static_cast<float>(w), -1.0f) * 0.5f;
+  float py = __fmaf_rn(__fadd_rn(gy, 1.0f), static_cast<float>(h), -1.0f) * 0.5f;
   px = fminf(fmaxf(px, 0.f), static_cast<float>(w - 1));
   py = fminf(fmaxf(py, 0.f), static_cast<float>(h - 1));
   const float x0f = floorf(px), y0f = floorf(py);

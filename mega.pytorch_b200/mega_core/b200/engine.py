@@ -1976,8 +1976,8 @@ class DffEngine(HeadCommon, MlpHeadMixin):
     the key frame's feature map along the flow, multiplies it by FlowNetS's scale map (one kernel, csrc/fgfa.cu) and
     feeds the single-frame RPN + box head (ResNetConv52MLPFeatureExtractor without channel reduction).
     Built from the FGFA parts (FlowNetS over row-slab / parity-class implicit GEMMs, pooled-image ring, pair builder).
-    NOT YET RUN ON A GPU (written after the last GPU session of round 1); parity test in tests/test_zz_train_ops_gpu.py
-    against the fixture of the unmodified reference (tests/golden/dff_r101_192x320.pt)."""
+    Parity test in tests/test_zz_train_ops_gpu.py against the fixture of the unmodified reference
+    (tests/golden/dff_r101_192x320.pt); the warp-and-scale kernel alone in tests/test_fgfa_conformance_gpu.py."""
 
     def __init__(self, sd, cfg=None, device="cuda"):
         cfg = cfg or EngineConfig()

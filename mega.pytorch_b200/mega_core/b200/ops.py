@@ -1170,15 +1170,33 @@ def vid_eval(det_boxes, det_scores, det_labels, det_offsets, det_scale, gt_boxes
 
 
 # --------------------------------------------------------------------------- FGFA helpers (csrc/fgfa.cu)
+# The kernels address an NHWC map as ((n * H + y) * W + x) * ld + channel with one ld per tensor (a ring slot or a flow
+# frame at slot * stride(0)), so every map they take must have unit channel stride and rows / images packed at that ld:
+# a cropped or transposed view would be read or written at the wrong pixels without any error.
 def _is16(t):
     return 1 if t.dtype == torch.float16 else 0
+
+
+def _rows_packed(t):
+    """t [..., H, W, C]: unit channel stride, stride(-3) == W * stride(-2) (any ld >= C, any outer stride)"""
+    h, w = t.shape[-3], t.shape[-2]
+    return t.stride(-1) == 1 and (h == 1 or t.stride(-3) == w * t.stride(-2))
+
+
+def _fgfa_fail(what, fmt, *args):
+    raise _lib.MegaError(what + ": " + fmt % args)
 
 
 def fgfa_pool_image(img, out):
     """img [1,3,H,W] or [3,H,W] fp32 -> out [ceil(H/2), ceil(W/2), 4] = avg_pool2d(img / 255, 2, ceil_mode)"""
     require_cuda(img, out)
     h, w = img.shape[-2:]
-    assert img.dtype == torch.float32 and img.is_contiguous()
+    if img.dtype != torch.float32 or not img.is_contiguous() or img.dim() < 3 or img.numel() != 3 * h * w:
+        _fgfa_fail("fgfa_pool_image", "img must be contiguous fp32 [3, H, W] (%s, %s)", img.dtype, tuple(img.shape))
+    if out.dtype not in (torch.float32, torch.float16) or not out.is_contiguous() or \
+            tuple(out.shape) != ((h + 1) // 2, (w + 1) // 2, 4):
+        _fgfa_fail("fgfa_pool_image", "out must be contiguous fp32 / fp16 [%d, %d, 4] (%s, %s)", (h + 1) // 2,
+                   (w + 1) // 2, out.dtype, tuple(out.shape))
     check(lib.mega_fgfa_pool_image(ptr(img), h, w, ptr(out), _is16(out), stream_ptr()), "mega_fgfa_pool_image")
     LAUNCHES[0] += 1
     return out
@@ -1189,6 +1207,14 @@ def fgfa_build_pairs(ring, slots, key_pos, pairs):
     require_cuda(ring, slots, pairs)
     s, hq, wq, _ = ring.shape
     assert ring.dtype == pairs.dtype and slots.dtype == torch.int32
+    if ring.shape[3] != 4 or ring.stride(2) != 4 or not _rows_packed(ring):
+        _fgfa_fail("fgfa_build_pairs", "ring slots must be dense [hq, wq, 4] (%s, strides %s)", tuple(ring.shape),
+                   ring.stride())
+    if not slots.is_contiguous() or slots.dim() != 1:
+        _fgfa_fail("fgfa_build_pairs", "slots must be a contiguous int32 vector (%s)", tuple(slots.shape))
+    if not pairs.is_contiguous() or tuple(pairs.shape) != (slots.numel(), hq + 6, wq + 8, 8):
+        _fgfa_fail("fgfa_build_pairs", "pairs must be contiguous [%d, %d, %d, 8] (%s)", slots.numel(), hq + 6, wq + 8,
+                   tuple(pairs.shape))
     check(lib.mega_fgfa_build_pairs(ptr(ring), ring.stride(0), ptr(slots), slots.numel(), key_pos, hq, wq, ptr(pairs),
                                     _is16(ring), stream_ptr()), "mega_fgfa_build_pairs")
     LAUNCHES[0] += 1
@@ -1196,9 +1222,17 @@ def fgfa_build_pairs(ring, slots, key_pos, pairs):
 
 
 def avgpool2_nhwc(x, out):
+    """x [N, H, W, C] -> out [N, ceil(H/2), ceil(W/2), C]; both with unit channel stride and packed rows / images"""
     require_cuda(x, out)
     n, h, w, c = x.shape
-    assert x.dtype == out.dtype and x.stride(3) == 1 and out.stride(3) == 1
+    assert x.dtype == out.dtype
+    ho, wo = (h + 1) // 2, (w + 1) // 2
+    for name, t, hh, ww in (("x", x, h, w), ("out", out, ho, wo)):
+        if not _rows_packed(t) or (t.shape[0] > 1 and t.stride(0) != hh * ww * t.stride(2)):
+            _fgfa_fail("avgpool2_nhwc", "%s must be NHWC with packed rows and images (%s, strides %s)", name,
+                       tuple(t.shape), t.stride())
+    if tuple(out.shape) != (n, ho, wo, c):
+        _fgfa_fail("avgpool2_nhwc", "out must be [%d, %d, %d, %d] (%s)", n, ho, wo, c, tuple(out.shape))
     check(lib.mega_avgpool2_nhwc(ptr(x), n, h, w, c, x.stride(2), ptr(out), out.stride(2), _is16(x), stream_ptr()),
           "mega_avgpool2_nhwc")
     LAUNCHES[0] += 1
@@ -1206,23 +1240,47 @@ def avgpool2_nhwc(x, out):
 
 
 def fgfa_aggregate(ring, slots, key_pos, flow, out, feat_channels, embed_channels, weights_out=None):
-    """ring [S, h, w, ld] ([feats | embeds] per pixel); flow [L, h, w, fl] fp32; out [h, w, >= feat_channels]"""
+    """ring [S, h, w, >= cf + ce] ([feats | embeds] per pixel); slots int32 [L]; flow [>= L, h, w, >= 2] fp32;
+    out [h, w, >= feat_channels]; weights_out [L, h, w] fp32"""
     require_cuda(ring, slots, flow, out, weights_out)
-    s, h, w, ld = ring.shape
+    s, h, w, _ = ring.shape
+    n = slots.numel()
     assert flow.dtype == torch.float32 and ring.dtype == out.dtype
-    check(lib.mega_fgfa_aggregate(ptr(ring), ring.stride(0), ld, feat_channels, embed_channels, ptr(slots), slots.numel(),
-                                  key_pos, ptr(flow), flow.stride(2), h, w, ptr(out), out.stride(-2), ptr(weights_out),
+    what = "fgfa_aggregate"
+    if not _rows_packed(ring) or feat_channels <= 0 or embed_channels <= 0 or \
+            feat_channels + embed_channels > ring.shape[3]:
+        _fgfa_fail(what, "ring must hold %d + %d channels with packed rows (%s, strides %s)", feat_channels,
+                   embed_channels, tuple(ring.shape), ring.stride())
+    if slots.dtype != torch.int32 or not slots.is_contiguous() or slots.dim() != 1:
+        _fgfa_fail(what, "slots must be a contiguous int32 vector (%s, %s)", slots.dtype, tuple(slots.shape))
+    if flow.dim() != 4 or flow.shape[0] < n or tuple(flow.shape[1:3]) != (h, w) or flow.shape[3] < 2 or \
+            not _rows_packed(flow) or (flow.shape[0] > 1 and flow.stride(0) != h * w * flow.stride(2)):
+        _fgfa_fail(what, "flow must be fp32 [>= %d, %d, %d, >= 2] with packed rows and frames (%s, strides %s)", n, h, w,
+                   tuple(flow.shape), flow.stride())
+    if out.dim() != 3 or tuple(out.shape[:2]) != (h, w) or out.shape[2] < feat_channels or not _rows_packed(out):
+        _fgfa_fail(what, "out must be [%d, %d, >= %d] with packed rows (%s, strides %s)", h, w, feat_channels,
+                   tuple(out.shape), out.stride())
+    if weights_out is not None and (weights_out.dtype != torch.float32 or not weights_out.is_contiguous() or
+                                    tuple(weights_out.shape) != (n, h, w)):
+        _fgfa_fail(what, "weights_out must be contiguous fp32 [%d, %d, %d] (%s, %s)", n, h, w, weights_out.dtype,
+                   tuple(weights_out.shape))
+    check(lib.mega_fgfa_aggregate(ptr(ring), ring.stride(0), ring.stride(2), feat_channels, embed_channels, ptr(slots),
+                                  n, key_pos, ptr(flow), flow.stride(2), h, w, ptr(out), out.stride(1), ptr(weights_out),
                                   _is16(ring), stream_ptr()), "mega_fgfa_aggregate")
     LAUNCHES[0] += 1
     return out
 
 
 def dff_warp_scale(key_feats, flow, scale, out):
-    """key_feats [h, w, C]; flow [h, w, fl] fp32 (x, y in cells); scale [h, w, >=C]; out [h, w, >=C] = warp(key_feats) * scale"""
+    """key_feats [h, w, C]; flow [h, w, fl >= 2] fp32 (x, y in cells); scale [h, w, >=C]; out [h, w, >=C]
+    = warp(key_feats) * scale"""
     require_cuda(key_feats, flow, scale, out)
     h, w, c = key_feats.shape
     assert flow.dtype == torch.float32 and key_feats.dtype == scale.dtype == out.dtype
-    assert key_feats.stride(2) == 1 and scale.stride(2) == 1 and out.stride(2) == 1 and key_feats.stride(0) == w * key_feats.stride(1)
+    for name, t, cmin in (("key_feats", key_feats, c), ("flow", flow, 2), ("scale", scale, c), ("out", out, c)):
+        if t.dim() != 3 or tuple(t.shape[:2]) != (h, w) or t.shape[2] < cmin or not _rows_packed(t):
+            _fgfa_fail("dff_warp_scale", "%s must be [%d, %d, >= %d] with packed rows (%s, strides %s)", name, h, w, cmin,
+                       tuple(t.shape), t.stride())
     check(lib.mega_dff_warp_scale(ptr(key_feats), key_feats.stride(1), c, ptr(flow), flow.stride(1), ptr(scale),
                                   scale.stride(1), h, w, ptr(out), out.stride(1), _is16(key_feats), stream_ptr()),
           "mega_dff_warp_scale")
