@@ -18,8 +18,8 @@ namespace mega {
 // Sigmoid focal loss (SigmoidFocalLoss_cuda.cu:20-103) through the log-sigmoid identities
 //     log p = -softplus(-x),   log(1 - p) = -softplus(x),   softplus(x) = max(x, 0) + log1p(exp(-|x|)),
 // i.e. ONE exp and ONE log1p per logit (+ the two powers) instead of three exps and two logs; p itself comes from the same
-// e = exp(-|x|). One thread handles four consecutive logits of a row when the class count allows it (128-bit loads /
-// stores); the target of a row is read once per thread.
+// e = exp(-|x|). One thread handles four consecutive logits of a row when the class count and the pointers' alignment
+// allow it (128-bit loads / stores); the target of a row is read once per thread.
 struct FocalTerms {
   float p, log_p, log_1mp;
 };
@@ -49,15 +49,16 @@ __device__ __forceinline__ float focal_bwd_one(float x, int t, int d, float gamm
   return 0.f;
 }
 
-template <bool BWD>
+// VEC: one thread per four consecutive logits of a row (128-bit loads / stores). The host picks it only when the class
+// count is a multiple of 4 (a float4 never straddles two rows) and logits, d_losses and out are 16-byte aligned.
+template <bool BWD, bool VEC>
 __global__ void focal_loss_kernel(long long total, const float* __restrict__ logits, const int* __restrict__ targets,
                                   const float* __restrict__ d_losses, int num_classes, float gamma, float alpha,
                                   float* __restrict__ out) {
-  const bool vec = (num_classes & 3) == 0;       // a float4 never straddles two rows
-  const long long items = vec ? total / 4 : total;
+  const long long items = VEC ? total / 4 : total;
   for (long long it = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; it < items;
        it += static_cast<long long>(gridDim.x) * blockDim.x) {
-    if (vec) {
+    if (VEC) {
       const long long i = it * 4;
       const long long n = i / num_classes;
       const int d = static_cast<int>(i - n * num_classes);
@@ -321,28 +322,36 @@ static int grid_dcn(long long total, int block) {
 
 using namespace mega;
 
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+template <bool BWD>
+static int focal_loss_launch(const float* logits, const int* targets, const float* d_losses, int num_samples,
+                             int num_classes, float gamma, float alpha, float* out, cudaStream_t stream) {
+  const long long total = static_cast<long long>(num_samples) * num_classes;
+  if (total == 0) return MEGA_OK;
+  const bool vec = (num_classes & 3) == 0 && aligned16(logits) && aligned16(out) && (!BWD || aligned16(d_losses));
+  if (vec)
+    focal_loss_kernel<BWD, true><<<grid_dcn(total / 2, 256), 256, 0, stream>>>(total, logits, targets, d_losses,
+                                                                               num_classes, gamma, alpha, out);
+  else
+    focal_loss_kernel<BWD, false><<<grid_dcn(total / 2, 256), 256, 0, stream>>>(total, logits, targets, d_losses,
+                                                                                num_classes, gamma, alpha, out);
+  MEGA_CUDA_CHECK(cudaGetLastError());
+  return MEGA_OK;
+}
+
 extern "C" int mega_sigmoid_focalloss_forward(const float* logits, const int* targets, int num_samples,
                                               int num_classes, float gamma, float alpha, float* losses,
                                               void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  const long long total = static_cast<long long>(num_samples) * num_classes;
-  if (total == 0) return MEGA_OK;
-  focal_loss_kernel<false><<<grid_dcn(total / 2, 256), 256, 0, stream>>>(total, logits, targets, nullptr, num_classes,
-                                                                         gamma, alpha, losses);
-  MEGA_CUDA_CHECK(cudaGetLastError());
-  return MEGA_OK;
+  return focal_loss_launch<false>(logits, targets, nullptr, num_samples, num_classes, gamma, alpha, losses,
+                                  static_cast<cudaStream_t>(stream_v));
 }
 
 extern "C" int mega_sigmoid_focalloss_backward(const float* logits, const int* targets, const float* d_losses,
                                                int num_samples, int num_classes, float gamma, float alpha,
                                                float* d_logits, void* stream_v) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  const long long total = static_cast<long long>(num_samples) * num_classes;
-  if (total == 0) return MEGA_OK;
-  focal_loss_kernel<true><<<grid_dcn(total / 2, 256), 256, 0, stream>>>(total, logits, targets, d_losses, num_classes,
-                                                                        gamma, alpha, d_logits);
-  MEGA_CUDA_CHECK(cudaGetLastError());
-  return MEGA_OK;
+  return focal_loss_launch<true>(logits, targets, d_losses, num_samples, num_classes, gamma, alpha, d_logits,
+                                 static_cast<cudaStream_t>(stream_v));
 }
 
 extern "C" int mega_deform_im2col(const float* input, const float* offset, const float* mask, int batch, int channels,

@@ -111,12 +111,19 @@ def _deform_conv(input, weight, bias, offset, mask, output, kh, kw, sh, sw, ph, 
     cog = cout // group
     if kg % 4 or cog % 4:
         raise RuntimeError("deform_conv (B200 build): per-group C*kh*kw and Cout must be multiples of 4")
+    if output.dtype != torch.float32 or not output.is_contiguous() or tuple(output.shape) != (b, cout, ho, wo):
+        raise RuntimeError("deform_conv: output must be a contiguous float32 tensor of shape %s, got %s %s" % (
+            (b, cout, ho, wo), output.dtype, tuple(output.shape)))
     kpad = c * kh * kw
     cols = torch.empty(b, ho * wo, kpad, device=input.device)
-    _lib.check(_lib.lib.mega_deform_im2col(_lib.ptr(input.float()), _lib.ptr(offset.contiguous().float()),
-                                           _lib.ptr(mask.contiguous().float()) if mask is not None else None, b, c, h,
-                                           w, kh, kw, ph, pw, sh, sw, dh, dw, deformable_group, kpad, _lib.ptr(cols),
-                                           _lib.stream_ptr()), "mega_deform_im2col")
+    # the converted operands stay bound until the launch is enqueued: a temporary freed earlier could be handed to the
+    # next conversion by the caching allocator, and the kernel would read one operand through another's pointer
+    x = input.float()
+    off = offset.contiguous().float()
+    msk = mask.contiguous().float() if mask is not None else None
+    _lib.check(_lib.lib.mega_deform_im2col(_lib.ptr(x), _lib.ptr(off), _lib.ptr(msk), b, c, h, w, kh, kw, ph, pw, sh,
+                                           sw, dh, dw, deformable_group, kpad, _lib.ptr(cols), _lib.stream_ptr()),
+               "mega_deform_im2col")
     nhwc = torch.empty(b, 1, ho * wo, cout, device=input.device)
     w2 = weight.float().reshape(cout, kg)
     for g in range(group):
@@ -152,10 +159,17 @@ def deform_psroi_pooling_forward(input, bbox, trans, out, top_count, no_trans, s
     if not input.is_contiguous():
         raise RuntimeError("input must be contiguous")
     n, c, h, w = input.shape
+    shape = (bbox.shape[0], int(output_dim), int(pooled_size), int(pooled_size))
+    for name, t in (("out", out), ("top_count", top_count)):
+        _writable(name, t)
+        if tuple(t.shape) != shape:
+            raise RuntimeError("%s must have shape %s, got %s" % (name, shape, tuple(t.shape)))
     num_classes = 1 if no_trans else trans.shape[1] // 2
+    x = input.float()
+    rois = bbox.contiguous().float()
     tr = trans.contiguous().float() if not no_trans else None
     _lib.check(_lib.lib.mega_deform_psroi_pooling_forward(
-        _lib.ptr(input.float()), _lib.ptr(bbox.contiguous().float()), _lib.ptr(tr), bbox.shape[0], c, h, w,
+        _lib.ptr(x), _lib.ptr(rois), _lib.ptr(tr), bbox.shape[0], c, h, w,
         int(bool(no_trans)), float(spatial_scale), int(output_dim), int(group_size), int(pooled_size), int(part_size),
         int(sample_per_part), float(trans_std), num_classes, _lib.ptr(out), _lib.ptr(top_count), _lib.stream_ptr()),
         "mega_deform_psroi_pooling_forward")
@@ -335,8 +349,11 @@ def deform_psroi_pooling_backward(out_grad, input, bbox, trans, top_count, input
     if not no_trans:
         _writable("trans_grad", trans_grad)
         tr, tg = trans.contiguous().float(), trans_grad
+    og = out_grad.float()
+    x = input.float()
+    rois = bbox.contiguous().float()
+    cnt = top_count.contiguous().float()
     _lib.check(_lib.lib.mega_deform_psroi_pooling_backward(
-        _lib.ptr(out_grad.float()), _lib.ptr(input.float()), _lib.ptr(bbox.contiguous().float()), _lib.ptr(tr),
-        _lib.ptr(top_count.contiguous().float()), bbox.shape[0], c, h, w, int(bool(no_trans)), float(spatial_scale),
+        _lib.ptr(og), _lib.ptr(x), _lib.ptr(rois), _lib.ptr(tr), _lib.ptr(cnt), bbox.shape[0], c, h, w, int(bool(no_trans)), float(spatial_scale),
         int(output_dim), int(group_size), int(pooled_size), int(part_size), int(sample_per_part), float(trans_std),
         num_classes, _lib.ptr(input_grad), _lib.ptr(tg), _lib.stream_ptr()), "mega_deform_psroi_pooling_backward")
